@@ -11,13 +11,15 @@ A "step" = one decode iteration of the schedule pushed through the hot path for 
     prepare_metadata  ->  per layer: fused qk-norm+RoPE  ->  attention (+ fused KV append)
 driven the way the reference's engine drives its backend (static buffers + CUDA-graph replay,
 engine/graph.py:105-158).  K timed steps are spread evenly over the 1023 decode iterations.
-Each layer has its own pool slice, so one step touches ~13 GB >> 126 MB of L2.
+Each layer has its own pool slice, so one step reads gigabytes, far more than the 50 MB L2 of an H100.
 
-Prints ONE JSON line (see the driver contract): value = decode tokens/s (device-timed, inputs
+Prints ONE JSON line: value = decode tokens/s (device-timed, inputs
 resident), e2e = same through the plugin API with host buffers, roofline for the decode kernel,
 cpu_baseline (the oracle on the host cores, bounded sample), prefill TFLOP/s as an extra key.
 `--impl reference` times the CPU oracle (the reference has no CPU implementation of this path,
 its arithmetic is CUDA-only FlashInfer; see DESIGN.md) on the same workload.
+`--dump-outputs DIR` writes what the last timed step computed (see dump_outputs) so that two builds can
+be compared output for output; the inputs are seeded, so the same arguments give the same inputs.
 """
 
 from __future__ import annotations
@@ -29,6 +31,7 @@ import json
 import os
 import random
 import sys
+import tempfile
 import threading
 import time
 from pathlib import Path
@@ -201,22 +204,17 @@ def effective_cpus() -> int:
     return max(1, min(n, 64))
 
 
-def load_ncu_traffic() -> dict:
-    """DRAM traffic of the dominant kernel from the committed `ncu --set full` capture
-    (profiles/r02_ncu_decode_tc_summary.json: one launch of tools/microbench.py decode, iteration 500)."""
-    p = ROOT / "profiles" / "r02_ncu_decode_tc_summary.json"
-    try:
-        d = json.loads(p.read_text())
-
-        def mb(key):
-            val, unit = d[key].split()[:2]
-            return float(val) * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}[unit]
-
-        return {"traffic": int(mb("dram__bytes_read.sum") + mb("dram__bytes_write.sum")),
-                "traffic_alg_bytes": 133917 * 4096 + 128 * (2 * 8 * 256 + 2 * 16 * 256),
-                "traffic_source": "profiles/r02_ncu_decode_tc_summary.json (ncu --set full, decode iteration 500, bs=128)"}
-    except Exception:
-        return {"traffic": None}
+def flashinfer_workspace() -> str:
+    """Where FlashInfer JIT-compiles (used when FLASHINFER_WORKSPACE_BASE is unset): the tree's
+    oracle/_ref/flashinfer_ws -- the cache tools/flashinfer_prebuild.py fills and the golden / in-situ tools
+    use -- when it exists and is writable, otherwise one fixed directory under the system temp dir, so that
+    a read-only tree stays untouched and repeated runs reuse their compiled modules."""
+    ws = ROOT / "oracle" / "_ref" / "flashinfer_ws"
+    if ws.is_dir() and os.access(ws, os.W_OK):
+        return str(ws)
+    tmp = Path(tempfile.gettempdir()) / f"mini-sglang-flashinfer-ws-{os.getuid()}"
+    tmp.mkdir(exist_ok=True)
+    return str(tmp)
 
 
 def load_peaks() -> dict:
@@ -225,7 +223,9 @@ def load_peaks() -> dict:
         d = json.loads(p.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1400.0, "source": "fallback"}
+    # NVIDIA's data sheet for the H100 SXM (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- a ceiling to
+    # divide by, not a rate any kernel reached
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data sheet"}
 
 
 # ----------------------------------------------------------------------------- clocks
@@ -351,6 +351,7 @@ class AttentionPathRunner:
         # are one contiguous block, so a step's host inputs arrive with ONE host-to-device copy
         self.qkv = torch.randn((self.n_seqs, L, self.width), device=device, dtype=torch.float32, generator=g).to(torch.bfloat16)
         self.last_out = {}
+        self.layer_outs = {}  # padded bs -> the captured graph's attention output of every layer
         self.positions = torch.zeros(self.n_seqs, dtype=torch.int32, device=device)
         self.out_loc = torch.zeros(self.n_seqs, dtype=torch.int32, device=device)
         self.qw = (torch.rand(D, device=device, generator=g) + 0.5).to(torch.bfloat16)
@@ -432,11 +433,14 @@ class AttentionPathRunner:
             self.stream.synchronize()
             g = torch.cuda.CUDAGraph()
             before = self.lib.b200_launch_count()
+            outs = []
             with torch.cuda.graph(g, stream=self.stream):
                 for l in range(L):
                     self.layer(l, bs, batch)
+                    outs.append(self._last_out)
             self.graph_launches[bs] = self.lib.b200_launch_count() - before
             self.last_out[bs] = self._last_out
+            self.layer_outs[bs] = outs
         self.graphs[bs] = g
 
     def schedule_step(self, triples):
@@ -467,8 +471,7 @@ class AttentionPathRunner:
                 self.copy_stream.wait_event(self.stg_free[slot])
                 with torch.cuda.stream(self.copy_stream):
                     # ALL host inputs of the step travel on the copy stream, the small index vectors first: a small
-                    # H2D on the compute stream would queue behind the 29 MB transfer in the DMA engine (that
-                    # head-of-line blocking cost ~1 ms per step, profiles/r02_e2e_probe.json)
+                    # H2D on the compute stream would queue behind the 29 MB transfer in the DMA engine
                     stg_idx[0, :bs].copy_(pos_h, non_blocking=True)
                     stg_idx[1, :bs].copy_(loc_h, non_blocking=True)
                     stg[:bs].copy_(qkv_h[:bs], non_blocking=True)
@@ -506,11 +509,41 @@ class AttentionPathRunner:
                 out_h[:bs].copy_(self.last_out[bs].view(bs, -1), non_blocking=True)
             # The step is over for the scheduler: its metadata dies with it, as in the engine, where a Batch does not
             # outlive its forward.  The timed steps are scheduled ahead of the timed region here; left alive, their
-            # metadata (slot-table snapshot, 1-2 MB each) made the caching allocator cudaMalloc a fresh segment every
-            # ~10 steps INSIDE the timed region: 0.3 ms as a rule, 5 ms .. 65 ms when the driver was busy (step 15 of
-            # every run, profiles/r02_stall_probe.txt) -- with 0.5 ms steps (one rank's shard of tp8) that was the run.
+            # metadata (slot-table snapshot, 1-2 MB each) would make the caching allocator cudaMalloc fresh segments
+            # INSIDE the timed region.
             batch.attn_metadata = None
         return n_tokens
+
+
+DUMP_MAX_BYTES = 64_000_000  # all files together, headers included (64 MB in either reading)
+
+
+def dump_outputs(runner: AttentionPathRunner, step, out_dir: str) -> None:
+    """What the last timed decode step computed, as a caller of the path receives it, in float32: the attention
+    output of every layer (attn_out.npy, [L, n, hq, D]) and the K / V rows the step appended to every layer's
+    pool slice (k_appended.npy / v_appended.npy, [L, n, hkv, D]; in the fused path k is the normed + roped row).
+    n = the step's real requests; when that would exceed 64 MB in all, a fixed seeded sample of them is written.
+    rows.npy lists the step's request rows that were written."""
+    batch, _, _, n = step
+    bs = batch.padded_size
+    torch.cuda.synchronize()
+    per_row = L * (runner.hq + 2 * runner.hkv) * D * 4 + 8  # the three arrays' rows + the row index
+    budget = DUMP_MAX_BYTES - 4 * 4096  # .npy headers
+    rows = np.arange(n)
+    if n * per_row > budget:
+        rows = np.sort(np.random.RandomState(0).choice(n, budget // per_row, replace=False))
+    idx = torch.from_numpy(rows).to(runner.dev)
+    loc = runner.out_loc[:bs][idx].long()
+    arrays = {
+        "attn_out": torch.stack([o.reshape(bs, runner.hq, D)[idx] for o in runner.layer_outs[bs]]),
+        "k_appended": torch.stack([runner.pool.k_cache(l).reshape(-1, runner.hkv, D)[loc] for l in range(L)]),
+        "v_appended": torch.stack([runner.pool.v_cache(l).reshape(-1, runner.hkv, D)[loc] for l in range(L)]),
+    }
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(out / f"{name}.npy", t.float().cpu().numpy())
+    np.save(out / "rows.npy", rows.astype(np.float64))
 
 
 def _parity_vs_gpu(a: torch.Tensor, b: torch.Tensor) -> float:
@@ -527,8 +560,9 @@ def ref_gpu_arms(runner, sched, pkg, peaks, iters, reps: int = 5, layers: int = 
     """The reference's two GPU attention paths timed beside ours in the same process, on the identical
     pool / page table / q (north_star: "next to the reference's own FlashInfer path on the same box ...
     in the same run"):  R-fi = FlashInfer fa2 wrappers with page_size 1 exactly as attention/fi.py:93-103,
-    134-165,185-188 calls them; R-trtllm = the TRT-LLM-gen sm100a cubins exactly as attention/trtllm.py:
-    57-89 calls them (what the reference auto-selects on B200, engine/engine.py:223-229).  `store_kv`
+    134-165,185-188 calls them; R-trtllm = the TRT-LLM-gen path exactly as attention/trtllm.py:57-89 calls
+    it -- only on compute capability 10.x, the only architecture FlashInfer ships its kernels for (elsewhere
+    it is neither timed nor compared, and its spread never enters a gate).  `store_kv`
     in front of both is our store kernel (the reference's tvm-ffi store.cu cannot be built offline; same
     bytes).  Per layer: [append +] attention, eager, layers on distinct pool slices (L2 cold), CUDA events,
     median of `reps`."""
@@ -536,7 +570,8 @@ def ref_gpu_arms(runner, sched, pkg, peaks, iters, reps: int = 5, layers: int = 
                  "parity_criterion": "oracle/tolerance.vs_reference_gpu: max (|a - b| - one output ulp)^+ / max|b|, pass <= 1.5e-3 "
                                      "(north_star 1e-3 + the fa2-vs-TRT-LLM-gen spread of the reference itself, keys *_parity_trtllm_vs_fi)"}
     try:
-        os.environ.setdefault("FLASHINFER_WORKSPACE_BASE", str(ROOT / "oracle" / "_ref" / "flashinfer_ws"))
+        if "FLASHINFER_WORKSPACE_BASE" not in os.environ:
+            os.environ["FLASHINFER_WORKSPACE_BASE"] = flashinfer_workspace()
         import flashinfer
         from flashinfer.decode import trtllm_batch_decode_with_kv_cache
         from flashinfer.prefill import trtllm_batch_context_with_kv_cache
@@ -546,8 +581,11 @@ def ref_gpu_arms(runner, sched, pkg, peaks, iters, reps: int = 5, layers: int = 
     nl = min(layers, L)
     scale = D**-0.5
     res["flashinfer"] = flashinfer.__version__
+    with_trtllm = torch.cuda.get_device_capability(dev)[0] == 10
+    if not with_trtllm:
+        res["trtllm"] = "not run: FlashInfer's TRT-LLM-gen kernels exist for compute capability 10.x only"
     ws_fi = torch.empty(128 * 1024 * 1024, dtype=torch.uint8, device=dev)
-    ws_trt = torch.zeros(128 * 1024 * 1024, dtype=torch.uint8, device=dev)
+    ws_trt = torch.zeros(128 * 1024 * 1024, dtype=torch.uint8, device=dev) if with_trtllm else None
 
     def timed(fn):
         ts = []
@@ -677,7 +715,8 @@ def ref_gpu_arms(runner, sched, pkg, peaks, iters, reps: int = 5, layers: int = 
                         kv_layout="NHD", out_dtype=torch.bfloat16)
 
             tag = f"decode_it{it}_bs{bs}"
-            outs, errs = run_three(tag, (("b200", ours), ("fi", fi), ("trtllm", trtllm)), nbytes, "GBs")
+            outs, errs = run_three(tag, (("b200", ours), ("fi", fi)) + ((("trtllm", trtllm),) if with_trtllm else ()),
+                                   nbytes, "GBs")
             torch.cuda.synchronize()
             try:
                 vs_oracle(tag, outs, errs, tr, nl - 1, qs[nl - 1][0])
@@ -730,7 +769,7 @@ def ref_gpu_arms(runner, sched, pkg, peaks, iters, reps: int = 5, layers: int = 
                     batch_size=len(trp), out_dtype=torch.bfloat16)
 
         tag = f"prefill_nnz{nnz}_reqs{len(trp)}"
-        run_three(tag, (("b200", ours_p), ("fi", fi_p), ("trtllm", trt_p)), flops, "TFs")
+        run_three(tag, (("b200", ours_p), ("fi", fi_p)) + ((("trtllm", trt_p),) if with_trtllm else ()), flops, "TFs")
     del ws_fi, ws_trt
     return res
 
@@ -806,17 +845,15 @@ def run_ours(args) -> dict:
         runner.decode_step(st)
     # A CUDA graph is uploaded to the device on its FIRST launch (milliseconds, and different on every rank): every
     # distinct captured graph the timed steps replay is launched once here, as a serving engine's graphs are warm
-    # after the first seconds (at tp8 a cold first launch per batch size cost more than the step itself and made
-    # the ranks' timed regions differ by 20 ms, profiles/r02_bench_tp8_cold_graphs.json).
+    # after the first seconds (a cold first launch per batch size can cost more than the step itself).
     seen_bs = set()
     for st in steps:
         if st[0].padded_size not in seen_bs:
             seen_bs.add(st[0].padded_size)
             runner.decode_step(st)
     # Python's cyclic collector is parked for the timed legs, as serving engines do after warm-up (gc.freeze): a
-    # full collection of a process with torch loaded takes 30-60 ms and the scheduler thread of this path is at
-    # most 4 steps (the pinned request ring) ahead of the GPU.  (Not what stalled the short-step runs of round 2 --
-    # that was cudaMalloc, see decode_step -- profiles/r02_stall_probe.txt has the A/B.)
+    # full collection of a process with torch loaded takes tens of milliseconds and the scheduler thread of this
+    # path is at most 4 steps (the pinned request ring) ahead of the GPU.
     if os.environ.get("B200_BENCH_KEEP_GC", "0") == "0":  # =1: A/B of the claim above
         gc.collect()
         gc.freeze()
@@ -849,6 +886,8 @@ def run_ours(args) -> dict:
     eager_launches = lib.b200_launch_count() - launches0
     graph_launches = sum(runner.graph_launches[runner.pad_bs(len(tr))] for tr in step_triples)
     value = tokens / (ms * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(runner, steps[-1], args.dump_outputs)
 
     # ---------------- host cost of a step with an idle GPU (no back-pressure from the pinned staging ring):
     # what the scheduler thread pays per decode iteration for prepare_metadata / prepare_for_replay / replay
@@ -925,7 +964,7 @@ def run_ours(args) -> dict:
     achieved = alg_bytes / (attn_ms * 1e-3) / 1e9
     roofline = {"kernel": "attn_decode_tc_kernel(+combine)", "bound": "hbm", "achieved": round(achieved, 1),
                 "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": round(achieved / peaks["hbm_gbs"], 4),
-                "peak_source": peaks["source"], **(load_ncu_traffic() if wl.name == "cfg1" and world == 1 else {"traffic": None}),
+                "peak_source": peaks["source"],
                 "alg_bytes_per_launch": int(alg_bytes / n_launch), "us_per_launch": round(attn_ms * 1e3 / n_launch, 2),
                 "per_step_bs_us_frac": per_step}
 
@@ -1035,7 +1074,7 @@ def run_ours(args) -> dict:
                                          "(csrc/allreduce.cu), one launch per layer inside the decode graph" % HIDDEN,
                                  "nccl": "nccl all-reduce [bs,%d] bf16 x %d per step (eager, behind the graph replay)" % (HIDDEN, L),
                                  "none": "none"}[runner.allreduce],
-                   "l2": "each layer reads its own pool slice; one step touches >> 126 MB L2",
+                   "l2": "each layer reads its own pool slice; one step touches far more than the 50 MB L2",
                    "hbm_roofline_tokens_per_s": round(ceiling, 1)},
         "frac_of_hbm_roofline": round(value / ceiling, 4),
         "e2e": {"value": round(e2e_value, 1), "unit": "tokens/s", "h2d_bytes_per_step": int(h2d / args.steps),
@@ -1209,6 +1248,8 @@ def main() -> None:
     ap.add_argument("--no-allreduce", action="store_true")
     ap.add_argument("--allreduce", default="b200", choices=["b200", "nccl"], help="TP all-reduce implementation (N > 1)")
     ap.add_argument("--opt", action="append", default=[], help="name=value for b200_set_option (A/B experiments)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32, at most 64 MB)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3

@@ -1,8 +1,8 @@
 /*
- * b200attn.h -- C ABI of the B200-native paged-attention backend for mini-sglang.
+ * b200attn.h -- C ABI of the H100-native paged-attention backend for mini-sglang.
  *
  * One shared library (libb200attn.so, built by mini-sglang_b200/build.py with
- * `nvcc -gencode arch=compute_100a,code=sm_100a`), plain pointers and sizes, no torch
+ * `nvcc -gencode arch=compute_90a,code=sm_90a`), plain pointers and sizes, no torch
  * types.  Every entry point enqueues work on the CUDA stream it is given and returns
  * immediately (never synchronises, CUDA-graph capturable).  Device pointers unless noted.
  *
@@ -42,19 +42,15 @@ B200_API const char* b200_build_digest(void);
 B200_API const char* b200_last_error(void);
 /* Number of kernels this library has launched so far (bench.py's gpu_launches). */
 B200_API uint64_t b200_launch_count(void);
-/* 1 if the library was compiled for sm_100a and the current device is CC 10.x. */
+/* 1 if the library was compiled for sm_90a and the current device is CC 9.x. */
 B200_API int b200_device_supported(void);
 /* Kernel selection knobs (debug / cross-checking only; defaults are the product path):
- *   "decode_impl": 1 = tcgen05 + TMA kernel (default), 0 = cp.async / CUDA-core kernel.
- *   "prefill_impl": 1 = tcgen05 kernel (default, needs prefill_plan), 0 = mma.sync bring-up kernel.
- *   "prefill_full_row": 1 = tcgen05 prefill with one softmax thread per query row (8 warps, whole score row in
- *       registers, setmaxnreg); 0 (default, measured faster) = two threads per row (16 warps).
- *   "decode_lookahead": S^T buffers the UMMA issuer may run ahead (2..4, default 4).
+ *   "decode_impl": 1 = wgmma + TMA kernel (default), 0 = cp.async / CUDA-core kernel.
+ *   "prefill_impl": 1 = wgmma kernel (default, needs prefill_plan), 0 = mma.sync bring-up kernel.
+ *   "prefill_order": 0 (default) = prefill work items size-sorted, heaviest first; 1 = request-major.
  *   "decode_fused_combine": 1 (default) = the chunk that arrives last merges the split-KV partials inside
  *       the decode launch (no combine launch), 0 = separate combine launch, 2 = in-kernel exactly when the
- *       plan policy leaves the batch unsplit (round 1's policy).
- *   "decode_defer_epilogue": 1 (default) = a decode unit's epilogue runs after the next unit's first
- *       tile has been handed to the tensor core; 0 = strictly unit after unit.
+ *       plan policy leaves the batch unsplit.
  *   "decode_early_kv": 1 (default) = a decode launch that is being captured into a CUDA graph lets its TMA
  *       producers stream K/V before the predecessor kernel has finished (programmatic dependent launch; the
  *       metadata and this layer's pool slice are not written inside the graph); 0 = always wait first.
@@ -205,7 +201,7 @@ B200_API int b200_attn_decode_fused(const void* q, int64_t q_row_stride, const v
 /* Prefill / extend: ragged query rows, cu_seqlens_q[bs+1]; request r has
  * q_len = cu_seqlens_q[r+1]-cu_seqlens_q[r] new tokens at kv positions
  * [seq_lens[r]-q_len, seq_lens[r]).  max_seqlen_q is a host-side upper bound (grid sizing).
- * prefill_plan: b200_build_prefill_plan output (work list of the tcgen05 kernel); NULL selects
+ * prefill_plan: b200_build_prefill_plan output (work list of the wgmma kernel); NULL selects
  * the mma.sync bring-up kernel (as does b200_set_option("prefill_impl", 0)). */
 B200_API int b200_attn_prefill(const void* q, int64_t q_row_stride, const void* k, int64_t k_row_stride,
                       const void* v, int64_t v_row_stride, void* k_cache, void* v_cache,

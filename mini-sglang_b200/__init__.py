@@ -1,4 +1,4 @@
-"""mini-sglang_b200 -- B200-native (sm_100a) paged-attention backend for mini-sglang.
+"""mini-sglang_b200 -- H100-native (sm_90a) paged-attention backend for mini-sglang.
 
 Holds only what the attention hot path needs (SURVEY.md section 8):
 

@@ -1,7 +1,7 @@
 """ctypes binding of libb200attn.so (the C ABI declared in ``include/b200attn.h``).
 
 The product path fails loudly when the native library is missing or the device is not
-sm_100: there is no CPU or PyTorch fallback anywhere below this module.
+sm_90: there is no CPU or PyTorch fallback anywhere below this module.
 """
 
 from __future__ import annotations
@@ -87,7 +87,7 @@ def load(path: Optional[os.PathLike] = None) -> C.CDLL:
     if not p.exists():
         raise B200NativeError(
             f"{p} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(there is no CPU fallback for the B200 attention path)"
+            "(there is no CPU fallback for the attention path)"
         )
     lib = C.CDLL(str(p))
     for name, (res, args) in SIGNATURES.items():

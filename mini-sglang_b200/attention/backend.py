@@ -1,5 +1,5 @@
 """``B200AttnBackend`` -- the drop-in ``BaseAttnBackend`` (reference ``python/minisgl/attention/
-base.py:18-34``) whose ``forward`` runs the hand-written sm_100a kernels of libb200attn.
+base.py:18-34``) whose ``forward`` runs the hand-written sm_90a kernels of libb200attn.
 
 Contract kept from the reference backends (fi.py:80-271, fa.py:36-136, trtllm.py:35-162):
 
@@ -174,8 +174,7 @@ class B200AttnBackend(BaseAttnBackend):
         """The request triples are written into one buffer of a small ring of PINNED host buffers and the
         metadata kernels read them from there directly (zero copy: pinned ``cudaHostAlloc`` memory is mapped
         into the device's unified address space) -- no host-to-device copy sits on the critical path of the
-        step, where it would queue behind any large upload in the DMA engine (measured: +1.1 ms per step
-        behind a 29 MB input upload, profiles/r02_e2e_probe.json).  The reference allocates a fresh pinned
+        step, where it would queue behind any large upload in the DMA engine.  The reference allocates a fresh pinned
         tensor and issues an H2D copy per step (fa.py:76-90).  Returns (device-visible pointer, event to
         record once the kernels that read it have been enqueued)."""
         n = len(flat)
@@ -299,7 +298,7 @@ class B200AttnBackend(BaseAttnBackend):
                 "b200_attn_decode",
             )
         else:
-            # Contract of the tcgen05 prefill kernel: it appends the tile that holds a unit's own tokens
+            # Contract of the wgmma prefill kernel: it appends the tile that holds a unit's own tokens
             # at slot_table[r, cached + i] (the metadata snapshot), which equals batch.out_loc by the
             # reference's construction out_loc = page_table[table_idx, cached_len:device_len]
             # (scheduler/scheduler.py:207-210); B200_DEBUG_CHECKS=1 verifies it per call (host sync).

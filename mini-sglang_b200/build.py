@@ -1,4 +1,4 @@
-"""Build libb200attn.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libb200attn.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
 The library is pure CUDA runtime + C ABI (``include/b200attn.h``): no torch headers, so a
 rebuild takes seconds and the product .so travels to the GPU box with the snapshot.
@@ -33,7 +33,7 @@ SOURCES = [
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-O3",
     "-std=c++17",
     "-lineinfo",
@@ -121,7 +121,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         _nvcc(),
         "-shared",
         "-gencode",
-        "arch=compute_100a,code=sm_100a",
+        "arch=compute_90a,code=sm_90a",
         "-o",
         str(LIB_PATH),
         *[str(o) for o in objs],

@@ -395,7 +395,7 @@ static int attn_decode_impl(const void* q, int64_t q_row_stride, const void* k,
                             slot_table, slot_table_stride, seq_lens, decode_plan, bs, hq, hkv, num_slots,
                             page_size, scale_log2, out, part_o, part_ml, counters, dtype, st, fuse, qw, kw,
                             eps, positions, cos_sin);
-  B200_CHECK_ARG(!fuse, "attn_decode_fused: only the tcgen05 kernel (decode_impl = 1) fuses qk-norm + RoPE");
+  B200_CHECK_ARG(!fuse, "attn_decode_fused: only the wgmma kernel (decode_impl = 1) fuses qk-norm + RoPE");
 #ifdef B200_BRINGUP_KERNELS
 #define FILL(T_)                                                                                  \
   DecodeParams<T_> p{(const T_*)q, q_row_stride, (const T_*)k, k_row_stride, (const T_*)v,        \

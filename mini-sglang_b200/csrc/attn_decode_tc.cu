@@ -1,35 +1,30 @@
-// Blackwell-native batched decode: TMA gather4 -> swizzled smem -> tcgen05 UMMA (TMEM accumulators).
+// Hopper-native batched decode: TMA -> 128B-swizzled smem -> wgmma (register accumulators).
 //
 // Replaces store_kv + BatchDecodeWithPagedKVCacheWrapper.run (python/minisgl/attention/fi.py:185-188)
 // with one persistent launch (+ the split-KV combine).  HBM-bound; algorithmic bytes as in
-// attn_decode.cu.  One CTA per SM, 384 threads, warp-specialised:
+// attn_decode.cu.  One CTA per SM, 320 threads, warp-specialised:
 //
-//   warps 0-3 TMA producers, 3-stage ring of 64 KB stages (K/V x two 64-column halves of a 128-key
-//            tile), data lands directly in the 128-byte-swizzled layout UMMA consumes.
-//            * page_size >= 8 ("box mode", warp 0 only): the slots of a page are contiguous rows of
-//              the pool, so one tiled TMA box of min(page_size, 64) rows x 128 B is issued per page
-//              piece -- 8 instructions per tile at page_size 64.  The one box of a request that
-//              straddles the end of its KV range falls back to gather4 with out-of-range rows
-//              (zero filled), so stale pool memory is never multiplied in.
-//            * page_size < 8 ("gather mode", all four warps): cp.async.bulk.tensor ...gather4, four
-//              arbitrary token rows per instruction, one instruction per lane per tile.
-//   warp 8   UMMA issuer (one thread):  S^T[128 keys x 16] = K_tile[128 x 128] . Q^T   (K-major A, B)
-//                                       O^T[128 dims x 16] = V_tile^T[128 x 128 keys] . P^T (MN-major A)
-//            i.e. the keys / head dims fill the M = 128 dimension and the <= 8 query heads of the
-//            GQA group sit in N = 16, so no tensor-core row is wasted on padding and the score
-//            tile comes out with one key per TMEM lane = one key per softmax thread.
-//   warp 9   Q loader: the group's q rows -> swizzled smem operand (double buffered across units);
-//            also owns the TMEM allocation (64 columns: 2 x S^T, 2 x O^T).
-//   warps 4-7 softmax + accumulation: thread i reads lane i of S^T (tcgen05.ld), the tile max is
-//            reduced with warp shuffles + one named barrier, P^T goes back to smem as the bf16 B
-//            operand, O^T tiles are read back and accumulated in registers with the online-softmax
-//            rescale; row sums are kept per thread and reduced once per unit.
+//   warps 0-3 TMA producers, 3-stage rings of 32 KB K and 32 KB V tiles (two 64-column halves of a
+//            128-key tile), data lands directly in the 128-byte-swizzled layout wgmma consumes.
+//            * page_size >= 8 ("box mode", warp 0 = K, warp 1 = V): the slots of a page are contiguous
+//              rows of the pool, so one tiled TMA box of min(page_size, 64) rows x 128 B is issued per
+//              page piece -- 4 instructions per tile and half at page_size 64.
+//            * page_size < 8 ("row mode", all four warps): one single-row TMA box per token row and
+//              half; rows past the end of the KV range are out-of-range rows (zero filled), so stale
+//              pool memory is never multiplied in.
+//   warps 4-7 one consumer warpgroup: S^T[128 keys x 8] = K_tile . Q^T and O^T[128 dims x 8] += V_tile^T . P^T
+//            as wgmma m64n8k16 (two 64-row blocks each): the keys / head dims fill M and the <= 8 query
+//            heads of the GQA group sit in N = 8, so no tensor-core row is spent on padding.  Softmax on
+//            the score fragments (tile max across the four warps through smem + a named barrier), P^T to
+//            smem as the 16-bit B operand, O^T stays in registers with the online-softmax rescale.
+//   warp 8   Q loader: the group's q rows -> swizzled smem operand (double buffered across units).
+//   warp 9   split-KV combiner: the last-arriving chunk of a (request, kv head) merges the partials.
 //
 // Fused pre-attention (p.fuse, b200_attn_decode_fused): q and the new k row arrive RAW (straight from the
 // qkv projection); the Q loader applies the per-head RMSNorm + neox RoPE of layers/attention.py:50-54 with
 // the arithmetic of qknorm_rope_kernel (qknorm_rope.cuh, bit for bit) while it builds the swizzled Q
 // operand, and hands the roped q / k rows the epilogue needs (new-token score, append payload) to the
-// softmax warps through a small smem ring -- the separate qk-norm + RoPE launch disappears and q / k are
+// consumer warps through a small smem ring -- the separate qk-norm + RoPE launch disappears and q / k are
 // never written back to global memory (only the pool row of the new token is).
 //
 // The token appended by this launch is handled without touching the pool copy that is being
@@ -39,7 +34,7 @@
 #include "combine.cuh"
 #include "common.cuh"
 #include "qknorm_rope.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 #include <type_traits>
 
@@ -50,21 +45,19 @@ int get_tensor_map_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
 
 namespace dtc {
 
-using namespace sm100;
+using namespace sm90;
 
 constexpr int kD = 128;
 constexpr int kTileN = 128;                 // keys per tile
 constexpr int kStages = 3;
-constexpr int kThreads = 384;
-constexpr int kWarpMma = 8, kWarpQ = 9, kWarpCombine = 10;
+constexpr int kThreads = 320;
+constexpr int kWarpQ = 8, kWarpCombine = 9;
 constexpr int kHalfBytes = kTileN * 128;    // one 64-column half of a K or V tile: 16 KB
 constexpr int kStageBytes = 2 * kHalfBytes; // one K (or V) tile: half 0 | half 1 = 32 KB
-constexpr int kQBufBytes = 2 * 2048;        // two halves of [16 rows x 128 B]
-constexpr int kPBufBytes = 16 * kTileN * 2; // P^T [16 x 128] bf16, no-swizzle K-major
-constexpr int kNPad = 16;                   // UMMA N (query heads of the group, padded)
-constexpr int kNumS = 4;                    // max S^T buffers in TMEM (QK^T look-ahead), runtime p.num_s
-constexpr int kTmemCols = 128;              // S^T: kNumS x 16 columns, O^T: 2 x 16 columns
-constexpr int kMaxUnitsSmem = 96;          // per-CTA work units decoded once into smem
+constexpr int kNPad = 8;                    // wgmma N (query heads of the group, padded)
+constexpr int kQBufBytes = 2 * 1024;        // two halves of [8 rows x 128 B], 128B-swizzled
+constexpr int kPBufBytes = kNPad * kTileN * 2;  // P^T [8 x 128] 16-bit, no-swizzle K-major
+constexpr int kMaxUnitsSmem = 96;           // per-CTA work units decoded once into smem
 constexpr int kEpiSlots = 4;                // fused mode: roped (q heads, new k) rows in flight to the epilogue
 constexpr int kEpiSlotBytes = 9 * kD * 2;   // up to 8 q heads + the k row, 128 x 16-bit each
 
@@ -74,16 +67,15 @@ struct Smem {
   static constexpr int vring = kStages * kStageBytes;      // V tiles, released after PV
   static constexpr int qbuf = 2 * kStages * kStageBytes;
   static constexpr int pbuf = qbuf + 2 * kQBufBytes;
-  static constexpr int bars = pbuf + 2 * kPBufBytes;      // 40 mbarriers
-  static constexpr int tmem_ptr = bars + 40 * 8;
-  static constexpr int red = tmem_ptr + 16;               // floats: [2][4][16] tile max, [2][4][16] row sums, [2][4][16] new-token dots
-  static constexpr int units = red + (2 * 4 * 16 + 2 * 4 * 16 + 2 * 4 * 16) * 4;  // decoded work units
+  static constexpr int bars = pbuf + kPBufBytes;           // 32 mbarriers
+  static constexpr int red = bars + 32 * 8;                // floats: tile max [4][8], [2][4][8] row sums, [2][4][8] new-token dots
+  static constexpr int units = red + (32 + 64 + 64) * 4;   // decoded work units
   static constexpr int epi = units + kMaxUnitsSmem * 40;   // fused mode: kEpiSlots x [9][128] 16-bit
   static constexpr int total = epi + kEpiSlots * kEpiSlotBytes;
 };
 static_assert(Smem::total + 1024 <= 232448, "decode kernel shared memory exceeds the 227 KB per-CTA limit");
-enum Bar { kFullK = 0, kEmptyK = 3, kFullV = 6, kEmptyV = 9, kSFull = 12, kPFull = 16, kOFull = 18, kQFull = 20, kQEmpty = 22, kFinFull = 24, kFinEmpty = 28, kEpiFull = 32, kEpiEmpty = 36 };
-constexpr int kFinRing = 4;  // units in flight between the softmax warps and the combiner warp
+enum Bar { kFullK = 0, kEmptyK = 3, kFullV = 6, kEmptyV = 9, kQFull = 12, kQEmpty = 14, kFinFull = 16, kFinEmpty = 20, kEpiFull = 24, kEpiEmpty = 28 };
+constexpr int kFinRing = 4;  // units in flight between the consumer warps and the combiner warp
 
 template <typename T>
 struct Params {
@@ -102,10 +94,8 @@ struct Params {
   const int32_t* plan;
   int bs, hq, hkv;
   int num_slots;
-  int box_rows;  // rows per tiled TMA box (8..64, divides page_size); 0 = gather4 mode
-  int num_s;     // S^T buffers in use (2..kNumS)
+  int box_rows;  // rows per tiled TMA box (8..64, divides page_size); 0 = row mode
   int fused_combine;  // 1: last-arriving unit merges the split-KV partials in this launch
-  int defer;          // 1: a unit's epilogue runs after the next unit's first P^T has been issued
   float scale_log2;
   T* out;
   float* part_o;
@@ -160,22 +150,20 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid / kWarp, lane = tid % kWarp;
   auto bar = [&](int i) { return sbase + Smem::bars + i * 8; };
-  volatile uint32_t* tmem_ptr_s = reinterpret_cast<volatile uint32_t*>(smem + Smem::tmem_ptr);
   float* red = reinterpret_cast<float*>(smem + Smem::red);
   uint8_t* sUnits = smem + Smem::units;
 
   // ---------------------------------------------------------------- setup that touches no global memory
-  // zero the operand buffers whose padding rows (heads >= G) are never written again
-  for (int i = tid; i < (2 * kQBufBytes + 2 * kPBufBytes) / 16; i += kThreads)
+  // zero the Q operand buffers whose padding rows (heads >= G) are never written again
+  for (int i = tid; i < (2 * kQBufBytes) / 16; i += kThreads)
     reinterpret_cast<uint4*>(smem + Smem::qbuf)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(bar(kFullK + s), 1);
-      mbar_init(bar(kEmptyK + s), 1);
+      mbar_init(bar(kEmptyK + s), 4);  // one elected arrival per consumer warp
       mbar_init(bar(kFullV + s), 1);
-      mbar_init(bar(kEmptyV + s), 1);
+      mbar_init(bar(kEmptyV + s), 4);
     }
-    for (int b = 0; b < kNumS; ++b) mbar_init(bar(kSFull + b), 1);
     for (int b = 0; b < kFinRing; ++b) {
       mbar_init(bar(kFinFull + b), 128);
       mbar_init(bar(kFinEmpty + b), 1);
@@ -185,10 +173,8 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       mbar_init(bar(kEpiEmpty + b), 1);
     }
     for (int b = 0; b < 2; ++b) {
-      mbar_init(bar(kPFull + b), 4);  // one elected arrival per softmax warp
-      mbar_init(bar(kOFull + b), 1);
       mbar_init(bar(kQFull + b), 1);
-      mbar_init(bar(kQEmpty + b), 1);
+      mbar_init(bar(kQEmpty + b), 4);
     }
     fence_barrier_init();
     prefetch_tensormap(&map_k);
@@ -196,14 +182,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     prefetch_tensormap(&box_k);
     prefetch_tensormap(&box_v);
   }
-  if (warp == kWarpQ) tmem_alloc(sbase + Smem::tmem_ptr, kTmemCols);
   // PDL: everything above may overlap the tail of the previous kernel in the stream.
   //  * p.early == 0 (eager launches): wait here -- from here on the results of every kernel before this one
   //    (in particular the metadata kernel's plan / seq_lens / slot table) are complete and visible.
   //  * p.early == 1 (launch captured into a CUDA graph): the metadata was written BEFORE the graph started
   //    (prepare_for_replay), and the K/V rows this launch streams belong to this layer's pool slice, which
   //    no other kernel of the graph writes -- so only the roles that consume the predecessor's outputs
-  //    (Q loader: q / k_new; softmax warps: v_new, out_loc operands, output / partial stores; combiner)
+  //    (Q loader: q / k_new; consumer warps: v_new, out_loc operands, output / partial stores; combiner)
   //    wait, while the TMA producers start streaming K/V at once: prologue, pipeline fill and the
   //    predecessor's tail (or a small kernel in between, e.g. the TP all-reduce) overlap.
   if (!p.early) pdl_wait();
@@ -235,16 +220,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     if (pos < total_units) u = get_unit(pos, p.hkv, chunk_tokens, order, seq_lens);
     return u;
   };
-  fence_proxy_async_smem();  // zero-fill above must be visible to UMMA operand reads
-  tc_fence_before_sync();
+  fence_proxy_async_smem();  // zero-fill above must be visible to wgmma operand reads
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_s;
   if (warp < 4) {
     // ============================================================ TMA producers
-    // K and V travel in separate rings (a K tile is dead as soon as QK^T has been issued, a V
+    // K and V travel in separate rings (a K tile is dead as soon as QK^T has completed, a V
     // tile only after PV), so each has its own producers: box mode warp 0 = K, warp 1 = V;
-    // gather mode warps 0,1 = K rows 0-63 / 64-127, warps 2,3 = V.
+    // row mode warps 0,1 = K rows 0-63 / 64-127, warps 2,3 = V.
     const int rb = p.box_rows;
     const int kind = rb > 0 ? warp : (warp >> 1);  // 0 = K, 1 = V
     if (rb > 0 && warp >= 2) {
@@ -275,7 +257,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           return rr;
         };
         if (rb == 0) {
-          // ---- gather mode: this warp owns 64 rows; lane = (row group, half)
+          // ---- row mode: this warp owns 64 rows; lane = (row group of four, half)
           const int grp = (warp & 1) * 16 + (lane >> 1), half = lane & 1;
           int4 nxt = make_int4(0, 0, 0, 0);
           if (u.n_tiles > 0) nxt = load_group(0, grp);
@@ -287,7 +269,12 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             if ((warp & 1) == 0 && lane == 0) mbar_arrive_expect_tx(bar(full0 + stage), kStageBytes);
             __syncwarp();
             const uint32_t dst = ring + stage * kStageBytes + half * kHalfBytes + grp * 512;
-            tma_gather4(dst, gmap, bar(full0 + stage), col0 + half * 64, cur.x, cur.y, cur.z, cur.w);
+            const uint32_t fb = bar(full0 + stage);
+            const int col = col0 + half * 64;
+            tma_load_2d(dst, gmap, fb, col, cur.x);
+            tma_load_2d(dst + 128, gmap, fb, col, cur.y);
+            tma_load_2d(dst + 256, gmap, fb, col, cur.z);
+            tma_load_2d(dst + 384, gmap, fb, col, cur.w);
           }
         } else {
           // ---- box mode: instruction idx = (box, half); a box is rb consecutive positions of one page
@@ -309,99 +296,11 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
               const int col = col0 + half * 64;
               // A box reaching past the end of the range still lies inside the request's page; the
               // extra K rows are masked by position and the extra V rows are zeroed in smem by the
-              // softmax warps before PV.  A box wholly past the end gets an out-of-range row => zeros.
+              // consumer warps before PV.  A box wholly past the end gets an out-of-range row => zeros.
               tma_load_2d(dst, bmap, fb, col, first_slot);
             }
           }
         }
-      }
-    }
-  } else if (warp == kWarpMma) {
-    // ============================================================ UMMA issuer (one thread)
-    if (lane == 0) {
-      constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, kNPad, kBf16, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, kNPad, kBf16, true, false);
-      // Two cursors walk the same unit/tile sequence: QK^T may run up to kNumS tiles (also across
-      // unit boundaries) ahead of PV, so K tiles are consumed -- and their ring slots recycled -- as
-      // soon as they land, independent of the softmax latency.
-      struct Cursor {
-        int k;           // round = index into this CTA's unit list
-        int j;           // tile within the unit
-        int n_tiles;     // tiles of the current unit
-        uint32_t tc;     // global tile counter
-        uint32_t uc;     // global counter of units with tiles
-      };
-      auto seek = [&](Cursor& c) {  // position on the next unit that has tiles
-        while (c.k < n_rounds) {
-          c.n_tiles = unit_at(c.k).n_tiles;
-          if (c.n_tiles > 0) return;
-          ++c.k;
-        }
-        c.n_tiles = 0;
-      };
-      auto advance = [&](Cursor& c) {
-        ++c.tc;
-        if (++c.j == c.n_tiles) {
-          c.j = 0;
-          ++c.uc;
-          ++c.k;
-          seek(c);
-        }
-      };
-      Cursor qk{0, 0, 0, 0, 0}, pv{0, 0, 0, 0, 0};
-      seek(qk);
-      seek(pv);
-      uint32_t spins = 0;
-      while (pv.k < n_rounds) {
-        bool progress = false;
-        // ---- S^T[tile] = K_tile . Q^T
-        if (qk.k < n_rounds && qk.tc - pv.tc < (uint32_t)p.num_s) {
-          const uint32_t tc = qk.tc, stage = tc % kStages, qb = qk.uc & 1;
-          if (mbar_test_wait(bar(kFullK + stage), (tc / kStages) & 1) &&
-              (qk.j > 0 || mbar_test_wait(bar(kQFull + qb), (qk.uc >> 1) & 1))) {
-            tc_fence_after_sync();
-            const uint32_t kb = sbase + Smem::kring + stage * kStageBytes;
-            const uint32_t qa = sbase + Smem::qbuf + qb * kQBufBytes;
-            const uint32_t d = tmem_base + (tc % p.num_s) * kNPad;
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk) {
-              const uint64_t da = make_smem_desc(kb + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
-              const uint64_t db = make_smem_desc(qa + (kk >> 2) * 2048 + (kk & 3) * 32, 16, 1024, kLayoutSW128);
-              umma_f16_ss(d, da, db, idesc_qk, kk > 0);
-            }
-            umma_commit(bar(kSFull + tc % p.num_s));
-            umma_commit(bar(kEmptyK + stage));  // the K tile is dead once these MMAs have read it
-            if (qk.j + 1 == qk.n_tiles) umma_commit(bar(kQEmpty + qb));  // last QK of the unit
-            advance(qk);
-            progress = true;
-          }
-        }
-        // ---- O^T[tile] = V_tile^T . P^T
-        if (pv.tc < qk.tc) {
-          const uint32_t tc = pv.tc, stage = tc % kStages;
-          if (mbar_test_wait(bar(kPFull + (tc & 1)), (tc >> 1) & 1) &&
-              mbar_test_wait(bar(kFullV + stage), (tc / kStages) & 1)) {
-            tc_fence_after_sync();
-            const uint32_t vb = sbase + Smem::vring + stage * kStageBytes;
-            const uint32_t pb = sbase + Smem::pbuf + (tc & 1) * kPBufBytes;
-            const uint32_t d = tmem_base + kNumS * kNPad + (tc & 1) * kNPad;
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk) {
-              // A = V^T (MN-major): 16 keys = two 8-key swizzle atoms of 1024 B; dims 64..127 at +16 KB
-              const uint64_t da = make_smem_desc(vb + kk * 2048, kHalfBytes, 1024, kLayoutSW128);
-              // B = P^T (K-major, no swizzle): 8x16-byte core matrices, k-chunks 128 B apart, n-groups 2 KB
-              const uint64_t db = make_smem_desc(pb + kk * 256, 128, 2048, kLayoutNone);
-              umma_f16_ss(d, da, db, idesc_pv, kk > 0);
-            }
-            umma_commit(bar(kOFull + (tc & 1)));
-            umma_commit(bar(kEmptyV + stage));
-            advance(pv);
-            progress = true;
-          }
-        }
-        if (progress) spins = 0;
-        else if (++spins > (1u << 28)) __trap();
       }
     }
   } else if (warp == kWarpQ) {
@@ -423,7 +322,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           const int g = idx >> 4, cc = idx & 15;
           const Vec8 v = *reinterpret_cast<const Vec8*>(p.q + (int64_t)u.r * p.q_rs +
                                                         (int64_t)(u.h * G + g) * kD + cc * 8);
-          *reinterpret_cast<Vec8*>(qdst + (cc >> 3) * 2048 + sw128_offset(g, cc & 7)) = v;
+          *reinterpret_cast<Vec8*>(qdst + (cc >> 3) * 1024 + sw128_offset(g, cc & 7)) = v;
         }
       } else {
         // per-head RMSNorm + RoPE on 16-lane groups, two rows per pass: the G q heads of the group and,
@@ -441,7 +340,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
                       : *reinterpret_cast<const Vec8*>(p.q + (int64_t)u.r * p.q_rs + (int64_t)(u.h * G + g) * kD + cc * 8);
           const Vec8 rv = qknorm_rope_lanes<T, 16, true>(xv, cc, is_k ? p.kw : p.qw, p.eps, cs_row, active);
           if (active) {
-            if (!is_k && need_q) *reinterpret_cast<Vec8*>(qdst + (cc >> 3) * 2048 + sw128_offset(g, cc & 7)) = rv;
+            if (!is_k && need_q) *reinterpret_cast<Vec8*>(qdst + (cc >> 3) * 1024 + sw128_offset(g, cc & 7)) = rv;
             if (need_epi) *reinterpret_cast<Vec8*>(edst + g * (kD * 2) + cc * 16) = rv;
           }
         }
@@ -456,44 +355,177 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       if (need_epi) ++epi_count;
     }
   } else if (warp >= 4 && warp < 8) {
-    // ============================================================ softmax / accumulate (128 threads)
+    // ============================================================ consumer warpgroup (128 threads)
     if (p.early) pdl_wait();
-    const int ct = tid - 128;          // 0..127 = TMEM lane = key within tile = output dim
-    const int cw = warp - 4;           // TMEM lane quadrant of this warp
-    const uint32_t lane_base = (uint32_t)(cw * 32) << 16;
-    float* red_max = red;              // [2][16 heads][4 warps], by tile parity
-    uint32_t tile_count = 0, fin_count = 0, unit_par = 0, epi_fin = 0;
-    // State of one unit's online softmax; everything the epilogue needs.
-    struct UnitState {
-      Unit u;
-      float l_thr[G], m_run[G], q_new[G], alpha_last[G];
-      float kn, vn;
-      int app_loc;
-      Vec8 app_x;
-      uint32_t last_tc;
-    };
-    float acc[G];  // O^T accumulator (thread = output dim); one unit at a time owns it
+    constexpr bool kTransV = true;  // A = V^T: the head dims (M) are the contiguous axis of a V tile
+    T* const tsel = nullptr;        // selects the bf16 / fp16 wgmma overload
+    const int ct = tid - 128;       // 0..127
+    const int cw = warp - 4;        // warp of the group
+    // accumulator fragment (see sm90.cuh): element i of 64-row block mb is row mb*64 + r0 + (i>>1)*8,
+    // column h0 + (i&1).  Rows are keys (S^T) or head dims (O^T), columns are the group's query heads.
+    const int r0 = 16 * cw + (lane >> 2), h0 = 2 * (lane & 3);
+    auto row_of = [&](int mb, int i) { return mb * 64 + r0 + ((i >> 1) << 3); };
+    float* red_max = red;          // [4 warps][8 heads]
+    float* red_sum0 = red + 32;    // [2 parity][4][8]
+    float* red_new0 = red + 96;    // [2 parity][4][8]
+    uint32_t tile_count = 0, q_count = 0, fin_count = 0, epi_fin = 0, unit_par = 0;
+    for (int k = 0; k < n_rounds; ++k) {
+      const Unit u = unit_at(k);
+      if (u.n_tiles < 0) continue;  // no unit for this CTA in the last round
+      float acc[2][4], l_thr[2], m_run[2];
 #pragma unroll
-    for (int g = 0; g < G; ++g) acc[g] = 0.f;
-
-    // acc = acc * a + O^T of tile tc (waits for that tile's PV MMA)
-    auto retire = [&](uint32_t tc, const float (&a)[G]) {
-      mbar_wait(bar(kOFull + (tc & 1)), (tc >> 1) & 1);
-      tc_fence_after_sync();
-      uint32_t o[16];
-      tmem_ld_x16(tmem_base + lane_base + kNumS * kNPad + (tc & 1) * kNPad, o);
-      tmem_wait_ld();
+      for (int e = 0; e < 2; ++e) {
+        l_thr[e] = 0.f;
+        m_run[e] = -INFINITY;
 #pragma unroll
-      for (int g = 0; g < G; ++g) acc[g] = acc[g] * a[g] + __uint_as_float(o[g]);
-    };
+        for (int i = 0; i < 4; ++i) acc[e][i] = 0.f;
+      }
+      // operands of the appended token's score / value (x = mb*2 + (i>>1) indexes this thread's four dims):
+      // issue the loads now, use them in the epilogue -- their latency hides behind the tile loop
+      float q_new[2][4], kn[4], vn[4];
+      int app_loc = 0;
+      Vec8 app_x = Vec8{{0u, 0u, 0u, 0u}};
+#pragma unroll
+      for (int x = 0; x < 4; ++x) {
+        kn[x] = vn[x] = 0.f;
+        q_new[0][x] = q_new[1][x] = 0.f;
+      }
+      if (u.last_chunk) {
+#pragma unroll
+        for (int x = 0; x < 4; ++x) {
+          const int dim = row_of(x >> 1, (x & 1) << 1);
+          if (!p.fuse) {  // fused mode: roped q / k come from the Q loader's ring in the epilogue
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (h0 + e < G)
+                q_new[e][x] = DTypeTraits<T>::to_float(p.q[(int64_t)u.r * p.q_rs + (int64_t)(u.h * G + h0 + e) * kD + dim]);
+            kn[x] = DTypeTraits<T>::to_float(p.k_new[(int64_t)u.r * p.k_rs + u.h * kD + dim]);
+          }
+          vn[x] = DTypeTraits<T>::to_float(p.v_new[(int64_t)u.r * p.v_rs + u.h * kD + dim]);
+        }
+        // fused KV append (threads 0-15: K row, 16-31: V row, 16 bytes each): destination slot and
+        // payload are fetched here as well, so the epilogue only issues the store
+        if (ct < 32) {
+          app_loc = p.out_loc[u.r];
+          const T* src = ct < 16 ? p.k_new + (int64_t)u.r * p.k_rs : p.v_new + (int64_t)u.r * p.v_rs;
+          if (!(p.fuse && ct < 16)) app_x = *reinterpret_cast<const Vec8*>(src + u.h * kD + (ct & 15) * 8);
+        }
+      }
+      if (u.n_tiles > 0) {
+        const uint32_t qb = q_count & 1;
+        mbar_wait(bar(kQFull + qb), (q_count >> 1) & 1);
+        const uint32_t qa = sbase + Smem::qbuf + qb * kQBufBytes;
+        for (int j = 0; j < u.n_tiles; ++j, ++tile_count) {
+          const uint32_t stage = tile_count % kStages, sphase = (tile_count / kStages) & 1;
+          // ---- S^T = K_tile . Q^T: A = K rows (K-major, 128B swizzle), B = Q rows (K-major)
+          mbar_wait(bar(kFullK + stage), sphase);
+          const uint32_t kb = sbase + Smem::kring + stage * kStageBytes;
+          float s[2][4];
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) s[mb][i] = 0.f;
+          wgmma_fence();
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk) {
+              const uint64_t da = make_smem_desc(kb + mb * 8192 + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
+              const uint64_t db = make_smem_desc(qa + (kk >> 2) * 1024 + (kk & 3) * 32, 16, 1024, kLayoutSW128);
+              wgmma_m64n8k16_ss<0>(s[mb], da, db, kk > 0, tsel);
+            }
+          wgmma_commit();
+          wgmma_wait0();
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(bar(kEmptyK + stage));                      // the K tile is dead
+            if (j + 1 == u.n_tiles) mbar_arrive(bar(kQEmpty + qb));  // last QK of the unit
+          }
+          const int n_valid = u.kv_end_tc - (u.kv_begin + j * kTileN);  // >= 1
+          if (p.box_rows > 0 && n_valid < kTileN) {
+            // box mode, last tile of the range: the V rows past the end hold whatever the page holds
+            // (possibly NaN bit patterns): zero them so that 0 * garbage cannot reach the output
+            mbar_wait(bar(kFullV + stage), sphase);
+            uint8_t* vt = smem + Smem::vring + stage * kStageBytes;
+            for (int idx = ct; idx < (kTileN - n_valid) * 16; idx += 128) {
+              const int row = n_valid + (idx >> 4), c16 = idx & 15;
+              *reinterpret_cast<uint4*>(vt + (c16 >> 3) * kHalfBytes + row * 128 + (c16 & 7) * 16) = make_uint4(0, 0, 0, 0);
+            }
+            fence_proxy_async_smem();
+          }
+          // ---- online softmax: per head (column) max over the 128 keys of the tile
+          float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const float v = row_of(mb, i) < n_valid ? s[mb][i] * p.scale_log2 : -INFINITY;
+              s[mb][i] = v;
+              mx[i & 1] = fmaxf(mx[i & 1], v);
+            }
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 4));
+            mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 8));
+            mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 16));
+          }
+          if (lane < 4) {
+            red_max[cw * 8 + h0] = mx[0];
+            red_max[cw * 8 + h0 + 1] = mx[1];
+          }
+          named_bar_sync(1, 128);
+          float alpha[2], psum[2] = {0.f, 0.f};
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int hh = h0 + e;
+            const float mt = fmaxf(fmaxf(red_max[hh], red_max[8 + hh]), fmaxf(red_max[16 + hh], red_max[24 + hh]));
+            const float m_new = fmaxf(m_run[e], mt);  // finite: every tile has >= 1 valid key
+            alpha[e] = fast_exp2(m_run[e] - m_new);
+            m_run[e] = m_new;
+          }
+          // P^T [head][key] as 8x8 core matrices (no swizzle, K-major): key chunks of 8 are 128 B apart
+          uint8_t* pdst = smem + Smem::pbuf;
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int key = row_of(mb, i), hh = h0 + (i & 1);
+              const float pv = fast_exp2(s[mb][i] - m_run[i & 1]);
+              psum[i & 1] += pv;
+              *reinterpret_cast<T*>(pdst + (key >> 3) * 128 + hh * 16 + (key & 7) * 2) = DTypeTraits<T>::from_float(pv);
+              acc[mb][i] *= alpha[i & 1];
+            }
+#pragma unroll
+          for (int e = 0; e < 2; ++e) l_thr[e] = l_thr[e] * alpha[e] + psum[e];
+          fence_proxy_async_smem();  // P^T (and zeroed V rows) visible to the tensor core
+          named_bar_sync(1, 128);    // every warp's P^T is written; the tile maxima may be overwritten
+          // ---- O^T += V_tile^T . P^T: A = V rows read MN-major, B = P^T (K-major, no swizzle)
+          mbar_wait(bar(kFullV + stage), sphase);
+          const uint32_t vb = sbase + Smem::vring + stage * kStageBytes;
+          const uint32_t pb = sbase + Smem::pbuf;
+          wgmma_fence();
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk) {
+              // 16 keys = two 8-key swizzle atoms of 1024 B; dims 64..127 in the second half (+16 KB)
+              const uint64_t da = make_smem_desc(vb + mb * kHalfBytes + kk * 2048, kHalfBytes, 1024, kLayoutSW128);
+              const uint64_t db = make_smem_desc(pb + kk * 256, 128, 1024, kLayoutNone);
+              wgmma_m64n8k16_ss<kTransV ? 1 : 0>(acc[mb], da, db, 1u, tsel);
+            }
+          wgmma_commit();
+          wgmma_wait0();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar(kEmptyV + stage));
+        }
+        ++q_count;
+      }
 
-    // Unit epilogue on CUDA cores: row sums, the appended token (score, value, pool append), output.
-    auto finish = [&](UnitState& st) {
-      const Unit& u = st.u;
-      // reduction scratch double buffered by unit parity: the next unit may write its slots while
-      // stragglers still read this unit's (every unit passes a named barrier in between)
-      float* red_sum = red + 2 * 4 * 16 + unit_par * 64;  // [4][16]
-      float* red_new = red + 4 * 4 * 16 + unit_par * 64;  // [4][16]
+      // ---- unit epilogue on CUDA cores: row sums, the appended token (score, value, pool append), output.
+      // Reduction scratch double buffered by unit parity: the next unit may write its slots while
+      // stragglers still read this unit's (every unit passes a named barrier in between).
+      float* red_sum = red_sum0 + unit_par * 32;
+      float* red_new = red_new0 + unit_par * 32;
       unit_par ^= 1;
       const bool epi = p.fuse && u.last_chunk;
       const uint32_t es = epi_fin % kEpiSlots;
@@ -503,69 +535,86 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
         ++epi_fin;
         const uint8_t* esrc = smem + Smem::epi + es * kEpiSlotBytes;
 #pragma unroll
-        for (int g = 0; g < G; ++g)
-          st.q_new[g] = DTypeTraits<T>::to_float(*reinterpret_cast<const T*>(esrc + g * (kD * 2) + ct * 2));
-        st.kn = DTypeTraits<T>::to_float(*reinterpret_cast<const T*>(esrc + G * (kD * 2) + ct * 2));
-        if (ct < 16) st.app_x = *reinterpret_cast<const Vec8*>(esrc + G * (kD * 2) + ct * 16);
-      }
-      float pnew[G];
+        for (int x = 0; x < 4; ++x) {
+          const int dim = row_of(x >> 1, (x & 1) << 1);
 #pragma unroll
-      for (int g = 0; g < G; ++g) {
-        const float ls = warp_sum(st.l_thr[g]);
-        float sn = 0.f;
-        if (u.last_chunk) sn = warp_sum(st.q_new[g] * st.kn);
-        if (lane == 0) {
-          red_sum[cw * 16 + g] = ls;
-          red_new[cw * 16 + g] = sn;
+          for (int e = 0; e < 2; ++e)
+            if (h0 + e < G) q_new[e][x] = DTypeTraits<T>::to_float(*reinterpret_cast<const T*>(esrc + (h0 + e) * (kD * 2) + dim * 2));
+          kn[x] = DTypeTraits<T>::to_float(*reinterpret_cast<const T*>(esrc + G * (kD * 2) + dim * 2));
+        }
+        if (ct < 16) app_x = *reinterpret_cast<const Vec8*>(esrc + G * (kD * 2) + ct * 16);
+      }
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float ls = l_thr[e], sn = 0.f;
+        if (u.last_chunk) sn = (q_new[e][0] * kn[0] + q_new[e][1] * kn[1]) + (q_new[e][2] * kn[2] + q_new[e][3] * kn[3]);
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) {
+          ls += __shfl_xor_sync(0xffffffffu, ls, o);
+          sn += __shfl_xor_sync(0xffffffffu, sn, o);
+        }
+        if (lane < 4) {
+          red_sum[cw * 8 + h0 + e] = ls;
+          red_new[cw * 8 + h0 + e] = sn;
         }
       }
       named_bar_sync(1, 128);
       if (epi && ct == 0) mbar_arrive(bar(kEpiEmpty + es));  // every thread has read its ring values
-      float l_tot[G];
+      float l_tot[2];
 #pragma unroll
-      for (int g = 0; g < G; ++g) {
-        l_tot[g] = red_sum[g] + red_sum[16 + g] + red_sum[32 + g] + red_sum[48 + g];
-        pnew[g] = 0.f;
+      for (int e = 0; e < 2; ++e) {
+        const int hh = h0 + e;
+        l_tot[e] = red_sum[hh] + red_sum[8 + hh] + red_sum[16 + hh] + red_sum[24 + hh];
       }
       if (u.last_chunk) {
 #pragma unroll
-        for (int g = 0; g < G; ++g) {
-          const float s_new = (red_new[g] + red_new[16 + g] + red_new[32 + g] + red_new[48 + g]) * p.scale_log2;
-          const float m_new = fmaxf(st.m_run[g], s_new);
-          const float a = fast_exp2(st.m_run[g] - m_new);
-          pnew[g] = fast_exp2(s_new - m_new);
-          acc[g] = acc[g] * a + pnew[g] * st.vn;
-          l_tot[g] = l_tot[g] * a + pnew[g];
-          st.m_run[g] = m_new;
+        for (int e = 0; e < 2; ++e) {
+          const int hh = h0 + e;
+          const float s_new = (red_new[hh] + red_new[8 + hh] + red_new[16 + hh] + red_new[24 + hh]) * p.scale_log2;
+          const float m_new = fmaxf(m_run[e], s_new);
+          const float a = fast_exp2(m_run[e] - m_new);
+          const float pnew = fast_exp2(s_new - m_new);
+#pragma unroll
+          for (int mb = 0; mb < 2; ++mb) {
+            acc[mb][e] = acc[mb][e] * a + pnew * vn[mb * 2];
+            acc[mb][2 + e] = acc[mb][2 + e] * a + pnew * vn[mb * 2 + 1];
+          }
+          l_tot[e] = l_tot[e] * a + pnew;
+          m_run[e] = m_new;
         }
         // fused KV append: this head's new K and V rows go into the pool (operands fetched at unit start)
         if (ct < 32) {
-          T* dst = (ct < 16 ? p.k_cache : p.v_cache) + (int64_t)st.app_loc * p.hkv * kD + u.h * kD + (ct & 15) * 8;
-          *reinterpret_cast<Vec8*>(dst) = st.app_x;
+          T* dst = (ct < 16 ? p.k_cache : p.v_cache) + (int64_t)app_loc * p.hkv * kD + u.h * kD + (ct & 15) * 8;
+          *reinterpret_cast<Vec8*>(dst) = app_x;
         }
       }
       // ---- write out
       if (u.n_chunks == 1) {
+        const float inv[2] = {1.f / l_tot[0], 1.f / l_tot[1]};
 #pragma unroll
-        for (int g = 0; g < G; ++g)
-          p.out[((int64_t)u.r * p.hq + u.h * G + g) * kD + ct] = DTypeTraits<T>::from_float(acc[g] / l_tot[g]);
+        for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            if (h0 + (i & 1) < G)
+              p.out[((int64_t)u.r * p.hq + u.h * G + h0 + (i & 1)) * kD + row_of(mb, i)] =
+                  DTypeTraits<T>::from_float(acc[mb][i] * inv[i & 1]);
       } else {
         const int64_t base = ((int64_t)u.r * kMaxSplits + u.c) * p.hq + u.h * G;
 #pragma unroll
-        for (int g = 0; g < G; ++g) p.part_o[(base + g) * kD + ct] = acc[g];
-        if (ct < G) {
-          // m_run / l_tot are uniform across threads; thread g stores head g's pair
-          float mm = 0.f, ll = 0.f;
+        for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-          for (int g = 0; g < G; ++g)
-            if (g == ct) {
-              mm = st.m_run[g];
-              ll = l_tot[g];
+          for (int i = 0; i < 4; ++i)
+            if (h0 + (i & 1) < G) p.part_o[(base + h0 + (i & 1)) * kD + row_of(mb, i)] = acc[mb][i];
+        if (cw == 0 && lane < 4) {
+          // m_run / l_tot of a head are uniform across threads; lanes 0-3 of warp 0 store heads h0, h0+1
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (h0 + e < G) {
+              p.part_ml[(base + h0 + e) * 2 + 0] = m_run[e];
+              p.part_ml[(base + h0 + e) * 2 + 1] = l_tot[e];
             }
-          p.part_ml[(base + ct) * 2 + 0] = mm;
-          p.part_ml[(base + ct) * 2 + 1] = ll;
         }
-        // ---- hand the unit to the combiner warp (asynchronous split-KV merge): the softmax warps
+        // ---- hand the unit to the combiner warp (asynchronous split-KV merge): the consumer warps
         // only pay an mbarrier arrive; the release/acquire pair orders the partial stores above
         // before the combiner's device-scope fence + arrival counter.
         if (p.fused_combine) {
@@ -575,128 +624,6 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           ++fin_count;
         }
       }
-#pragma unroll
-      for (int g = 0; g < G; ++g) acc[g] = 0.f;
-    };
-
-    // The last tile of a unit is retired, and the unit's epilogue run, only AFTER the first P^T of
-    // the next unit has been handed to the tensor core (p.defer): the PV latency of the last tile
-    // and the epilogue then overlap the next unit's first PV instead of idling the pipe.
-    UnitState cur, old;
-    bool pending = false;
-    for (int k = 0; k < n_rounds; ++k) {
-      cur.u = unit_at(k);
-      const Unit& u = cur.u;
-      if (u.n_tiles < 0) continue;  // no unit for this CTA in the last round
-      cur.kn = 0.f;
-      cur.vn = 0.f;
-      cur.app_loc = 0;
-      cur.app_x = Vec8{{0u, 0u, 0u, 0u}};
-#pragma unroll
-      for (int g = 0; g < G; ++g) {
-        cur.l_thr[g] = 0.f;
-        cur.m_run[g] = -INFINITY;
-        cur.alpha_last[g] = 0.f;
-        cur.q_new[g] = 0.f;
-      }
-      if (u.last_chunk) {
-        // operands of the appended token's score / value: issue the loads now, use them in the
-        // epilogue -- their latency hides behind the tile loop
-        if (!p.fuse) {  // fused mode: roped q / k come from the Q loader's ring in the epilogue
-          const T* qrow = p.q + (int64_t)u.r * p.q_rs + (int64_t)(u.h * G) * kD + ct;
-#pragma unroll
-          for (int g = 0; g < G; ++g) cur.q_new[g] = DTypeTraits<T>::to_float(qrow[g * kD]);
-          cur.kn = DTypeTraits<T>::to_float(p.k_new[(int64_t)u.r * p.k_rs + u.h * kD + ct]);
-        }
-        cur.vn = DTypeTraits<T>::to_float(p.v_new[(int64_t)u.r * p.v_rs + u.h * kD + ct]);
-        // fused KV append (threads 0-15: K row, 16-31: V row, 16 bytes each): destination slot and
-        // payload are fetched here as well, so the epilogue only issues the store
-        if (ct < 32) {
-          cur.app_loc = p.out_loc[u.r];
-          const T* src = ct < 16 ? p.k_new + (int64_t)u.r * p.k_rs : p.v_new + (int64_t)u.r * p.v_rs;
-          if (!(p.fuse && ct < 16)) cur.app_x = *reinterpret_cast<const Vec8*>(src + u.h * kD + (ct & 15) * 8);
-        }
-      }
-      if (u.n_tiles == 0) {
-        // nothing for the tensor core (the unit is just the appended token)
-        if (pending) {
-          retire(old.last_tc, old.alpha_last);
-          finish(old);
-          pending = false;
-        }
-        finish(cur);
-        continue;
-      }
-      for (int j = 0; j < u.n_tiles; ++j) {
-        const uint32_t tc = tile_count + j;
-        mbar_wait(bar(kSFull + tc % p.num_s), (tc / p.num_s) & 1);
-        tc_fence_after_sync();
-        uint32_t s[16];
-        tmem_ld_x16(tmem_base + lane_base + (tc % p.num_s) * kNPad, s);
-        tmem_wait_ld();
-        const int n_valid = u.kv_end_tc - (u.kv_begin + j * kTileN);  // >= 1
-        const bool valid = ct < n_valid;
-        if (p.box_rows > 0 && n_valid < kTileN) {
-          // box mode, last tile of the range: the V rows past the end hold whatever the page holds
-          // (possibly NaN bit patterns): zero them so that 0 * garbage cannot reach the output
-          const uint32_t stage = tc % kStages;
-          mbar_wait(bar(kFullV + stage), (tc / kStages) & 1);
-          uint8_t* vt = smem + Smem::vring + stage * kStageBytes;
-          for (int idx = ct; idx < (kTileN - n_valid) * 16; idx += 128) {
-            const int row = n_valid + (idx >> 4), c16 = idx & 15;
-            *reinterpret_cast<uint4*>(vt + (c16 >> 3) * kHalfBytes + row * 128 + (c16 & 7) * 16) = make_uint4(0, 0, 0, 0);
-          }
-        }
-        float sv[G];
-        float* rm = red_max + (tc & 1) * 64;
-#pragma unroll
-        for (int g = 0; g < G; ++g) {
-          sv[g] = valid ? __uint_as_float(s[g]) * p.scale_log2 : -INFINITY;
-          const float mx = warp_max_redux(sv[g]);
-          if (lane == 0) rm[g * 4 + cw] = mx;  // [head][warp]: the four warp maxima of a head are one 16-byte read
-        }
-        named_bar_sync(1, 128);
-        float alpha[G];
-        uint8_t* pdst = smem + Smem::pbuf + (tc & 1) * kPBufBytes;
-#pragma unroll
-        for (int g = 0; g < G; ++g) {
-          const float4 wm = *reinterpret_cast<const float4*>(rm + g * 4);
-          const float mt = fmaxf(fmaxf(wm.x, wm.y), fmaxf(wm.z, wm.w));
-          const float m_new = fmaxf(cur.m_run[g], mt);  // finite: every tile has >= 1 valid key
-          alpha[g] = fast_exp2(cur.m_run[g] - m_new);
-          const float pv = fast_exp2(sv[g] - m_new);
-          cur.l_thr[g] = cur.l_thr[g] * alpha[g] + pv;
-          cur.m_run[g] = m_new;
-          *reinterpret_cast<T*>(pdst + (g >> 3) * 2048 + (ct >> 3) * 128 + (g & 7) * 16 + (ct & 7) * 2) =
-              DTypeTraits<T>::from_float(pv);
-        }
-        fence_proxy_async_smem();   // P^T visible to the tensor core
-        tc_fence_before_sync();     // our tcgen05.ld of S^T is ordered before the next QK overwrite
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(kPFull + (tc & 1)));  // one arrival per warp instead of 32 smem atomics
-        if (j > 0) {
-          retire(tc - 1, cur.alpha_last);
-        } else if (pending) {
-          retire(old.last_tc, old.alpha_last);
-          finish(old);
-          pending = false;
-        }
-#pragma unroll
-        for (int g = 0; g < G; ++g) cur.alpha_last[g] = alpha[g];
-      }
-      tile_count += u.n_tiles;
-      cur.last_tc = tile_count - 1;
-      if (p.defer) {
-        old = cur;
-        pending = true;
-      } else {
-        retire(cur.last_tc, cur.alpha_last);
-        finish(cur);
-      }
-    }
-    if (pending) {
-      retire(old.last_tc, old.alpha_last);
-      finish(old);
     }
   } else if (warp == kWarpCombine) {
     // ============================================================ split-KV combiner (one warp)
@@ -786,12 +713,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   }
 
   // ---------------------------------------------------------------- teardown
-  tc_fence_before_sync();
   __syncthreads();
-  if (warp == kWarpQ) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 template <typename T, int G>
@@ -843,9 +765,7 @@ static int launch(const Params<T>& p, cudaStream_t st) {
 
 }  // namespace dtc
 
-extern std::atomic<int> g_decode_lookahead;
 extern std::atomic<int> g_decode_fused_combine;
-extern std::atomic<int> g_decode_defer;
 extern std::atomic<int> g_decode_early_kv;
 bool decode_plan_is_unsplit(int bs, int num_kv_heads, int ctas);  // metadata.cu
 
@@ -861,9 +781,6 @@ int launch_decode_tc(const void* q, int64_t q_rs, const void* k, int64_t k_rs, c
   // then; still correct for a foreign plan that does split) and skip the combine launch.
   int fused = g_decode_fused_combine.load();
   if (fused == 2) fused = decode_plan_is_unsplit(bs, hkv, 2 * num_sms()) ? 1 : 0;
-  int num_s = g_decode_lookahead.load();
-  if (num_s < 2) num_s = 2;
-  if (num_s > dtc::kNumS) num_s = dtc::kNumS;
   // rows per tiled TMA box: largest power of two <= min(page_size, 64) that divides page_size
   int box_rows = 0;
   if (page_size >= 8) {
@@ -884,7 +801,7 @@ int launch_decode_tc(const void* q, int64_t q_rs, const void* k, int64_t k_rs, c
 #define RUN(T_)                                                                                   \
   dtc::Params<T_> p{(const T_*)q, q_rs, (const T_*)k, k_rs, (const T_*)v, v_rs, (T_*)k_cache,     \
                     (T_*)v_cache, out_loc, slot_table, st_stride, seq_lens, plan, bs, hq, hkv,    \
-                    (int)num_slots, box_rows, num_s, fused, g_decode_defer.load(), scale_log2, (T_*)out,  \
+                    (int)num_slots, box_rows, fused, scale_log2, (T_*)out,                        \
                     part_o, part_ml, counters, early, fuse, (const T_*)qw, (const T_*)kw, eps, positions, cos_sin};  \
   return dtc::launch<T_>(p, st)
   if (dtype == B200_DTYPE_BF16) {

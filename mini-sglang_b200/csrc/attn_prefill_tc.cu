@@ -1,32 +1,26 @@
-// Blackwell-native ragged prefill / extend attention: TMA -> swizzled smem -> tcgen05 UMMA with
-// S, P and O resident in TMEM (replaces BatchPrefillWithPagedKVCacheWrapper.run,
-// python/minisgl/attention/fi.py:150-165,188; causal, bottom-right aligned).
+// Hopper-native ragged prefill / extend attention: TMA -> swizzled smem -> wgmma with S, P and O in
+// registers (replaces BatchPrefillWithPagedKVCacheWrapper.run, python/minisgl/attention/fi.py:150-165,188;
+// causal, bottom-right aligned).
 //
 // Compute-bound: exact causal flops = 4*Hq*D*sum_r[q*cached + q(q+1)/2].
-// Persistent, one CTA per SM, 640 threads.  A work unit is (request, 128-row query tile, kv head,
-// pair of query heads of that kv head's GQA group): the two heads ("sub-tiles" A and B) share every
-// K/V tile, so K/V bytes per flop are halved and two softmax warpgroups ping-pong against one
-// tensor pipe (FlashAttention-4 style):
+// Persistent, one CTA per SM, 384 threads = three warpgroups.  A work unit is (request, 128-row query
+// tile, query head); the query heads of one kv head are adjacent units, so neighbouring CTAs stream the
+// same K/V rows and the re-reads hit in L2.
 //
-//   warp 0      K producer (+ the unit's Q sub-tiles): TMA boxes per page piece / gather4 rows
+//   warp 0      K producer (+ the unit's Q tile): TMA boxes per page piece / single-row boxes
 //   warp 1      V producer
-//   (append)    fused KV append: before their first score tile arrives the softmax warps copy
-//               pool[out_loc[t]] = k[t], v[t]; the attention reads this forward's tokens from the
-//               k / v inputs, never back from the pool, so no ordering is needed
-//   warp 2      UMMA issuer (one thread) + TMEM allocation
-//                 S_s = Q_s . K^T            (A, B from smem, K-major, 128B swizzle)  128x128 fp32
-//                 O_s += P_s . V             (A = P_s from TMEM, B = V tile MN-major)  128x128 fp32
-//               issue order per KV tile j:  PV_A(j) QK_A(j+1) PV_B(j) QK_B(j+1)  (in-order tensor pipe)
-//   warps 4-19  softmax, 8 warps per sub-tile: two threads per query row (TMEM lane), one per half of
-//               the 128 score columns; they exchange only the tile's row max (smem + named barrier).
-//               exp2 / row sum per thread, P written back to TMEM as packed bf16 over the thread's own
-//               S columns, O rescaled in TMEM only when the running max moved by more than 2^8 (lazy
-//               correction), chunks of 32 columns that are fully masked for the whole warp are skipped,
-//               final O/l -> bf16 -> global.
-// TMEM: S_A 0..127 (P_A aliases 0..31 and 64..95), S_B 128..255, O_A 256..383, O_B 384..511.
+//   (append)    fused KV append: the producers write the tile of a unit that holds the unit's own new
+//               tokens to the pool straight from shared memory (TMA store); the attention reads this
+//               forward's tokens from the k / v inputs, never back from the pool, so no ordering is needed
+//   warps 4-7   consumer warpgroup 0: query rows 0-63 of the tile;  warps 8-11: rows 64-127
+//               S = Q . K^T      wgmma m64n128k16, A and B from smem (K-major, 128B swizzle), fp32 registers
+//               O += P . V       wgmma m64n128k16, A = P from registers (16-bit), B = V tile read MN-major
+//               online softmax on the score fragments: a query row lives in one quad of lanes, so the row
+//               max / sum need two shuffles; K/V tiles that are fully masked for all 64 rows are skipped.
+// The producer warpgroup hands registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 = 384 x 168.
 #include "b200attn.h"
 #include "common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 #include <type_traits>
 
@@ -37,31 +31,27 @@ int get_tensor_map_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
 
 namespace ptc {
 
-using namespace sm100;
+using namespace sm90;
 
 constexpr int kD = 128;
-constexpr int kBM = 128;                   // query rows per sub-tile
+constexpr int kBM = 128;                   // query rows per unit (two consumer warpgroups x 64)
 constexpr int kBN = 128;                   // keys per tile
 constexpr int kStages = 2;                 // K ring depth = V ring depth
-constexpr int kThreadsHalfRow = 640;       // 4 control warps + 16 softmax warps (two threads per query row)
-constexpr int kThreadsFullRow = 384;       // 4 control warps + 8 softmax warps (one thread per query row)
-constexpr int kHalfBytes = 128 * 128;      // [128 rows x 64 cols] bf16, 128B-swizzled: 16 KB
+constexpr int kThreads = 384;
+constexpr int kHalfBytes = 128 * 128;      // [128 rows x 64 cols] 16-bit, 128B-swizzled: 16 KB
 constexpr int kTileBytes = 2 * kHalfBytes; // 32 KB
 constexpr int kMaxUnitsSmem = 64;
-constexpr int kTmemCols = 512;
-constexpr float kRescaleThreshold = 8.0f;  // log2 domain
 
 struct Smem {
-  static constexpr int q = 0;                              // 2 sub-tiles x 32 KB
-  static constexpr int kring = 2 * kTileBytes;             // kStages x 32 KB
+  static constexpr int q = 0;                                // one 128-row Q tile: 32 KB
+  static constexpr int kring = kTileBytes;                   // kStages x 32 KB
   static constexpr int vring = kring + kStages * kTileBytes;
-  static constexpr int bars = vring + kStages * kTileBytes;  // 24 mbarriers
-  static constexpr int tmem_ptr = bars + 24 * 8;
-  static constexpr int red = tmem_ptr + 16;                 // [3][2 sub][2 half][128] floats
-  static constexpr int units = red + 3 * 2 * 2 * 128 * 4;
+  static constexpr int bars = vring + kStages * kTileBytes;  // 10 mbarriers
+  static constexpr int units = bars + 16 * 8;
   static constexpr int total = units + kMaxUnitsSmem * 48;
 };
-enum Bar { kFullK = 0, kEmptyK = 2, kFullV = 4, kEmptyV = 6, kQFull = 8, kQEmpty = 9, kSFull = 10, kPFull = 12, kOFull = 14 };
+static_assert(Smem::total + 1024 <= 232448, "prefill kernel shared memory exceeds the 227 KB per-CTA limit");
+enum Bar { kFullK = 0, kEmptyK = 2, kFullV = 4, kEmptyV = 6, kQFull = 8, kQEmpty = 9 };
 
 template <typename T>
 struct Params {
@@ -87,19 +77,17 @@ struct Params {
 };
 
 struct Unit {
-  int r, q_start, q_len, q_begin, kv_len, cached, kv_hi, n_tiles, h, head0, n_sub;
+  int r, q_start, q_len, q_begin, kv_len, cached, kv_hi, n_tiles, h, head, owner;
 };
 static_assert(sizeof(Unit) <= 48, "Unit must fit its smem slot");
 
-__device__ __forceinline__ Unit get_unit(int pos, int hkv, int group, const int32_t* items,
+__device__ __forceinline__ Unit get_unit(int pos, int hq, int group, const int32_t* items,
                                          const int32_t* seq_lens, const int32_t* cu_q) {
   Unit u;
-  const int n_pairs = (group + 1) >> 1;
-  const int per_item = hkv * n_pairs;
-  const int item = pos / per_item;
-  const int rem = pos - item * per_item;
-  u.h = rem / n_pairs;
-  const int pair = rem - u.h * n_pairs;
+  const int item = pos / hq;
+  u.head = pos - item * hq;
+  u.h = u.head / group;
+  u.owner = (u.head == u.h * group);  // the first query head of a kv head appends its rows
   const int e = items[item];
   u.r = e & 0xffff;
   u.q_start = ((e >> 16) & 0xffff) * kBM;
@@ -109,8 +97,6 @@ __device__ __forceinline__ Unit get_unit(int pos, int hkv, int group, const int3
   u.cached = u.kv_len - u.q_len;
   u.kv_hi = min(u.kv_len, u.cached + min(u.q_len, u.q_start + kBM));
   u.n_tiles = (u.kv_hi + kBN - 1) / kBN;
-  u.head0 = u.h * group + pair * 2;
-  u.n_sub = min(2, group - pair * 2);
   return u;
 }
 
@@ -120,25 +106,8 @@ __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-// tcgen05.ld of 32 columns into r[0..31] (a slice of a larger register array)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-
-// kFullRow = true: FlashAttention-4 style softmax -- ONE thread per query row (8 softmax warps, register
-// budget raised with setmaxnreg), the whole 128-column score row lives in registers: one TMEM read per
-// tile, no cross-thread max exchange, no named barrier inside the tile loop.
-// kFullRow = false: two threads per query row (16 softmax warps), the round-1 variant, kept for A/B runs.
-template <typename T, bool kFullRow>
-__global__ void __launch_bounds__(kFullRow ? kThreadsFullRow : kThreadsHalfRow, 1)
+template <typename T>
+__global__ void __launch_bounds__(kThreads, 1)
 attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map_q,
                        const __grid_constant__ CUtensorMap map_k,
                        const __grid_constant__ CUtensorMap map_v,
@@ -153,23 +122,21 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid / kWarp, lane = tid % kWarp;
   auto bar = [&](int i) { return sbase + Smem::bars + i * 8; };
-  volatile uint32_t* tmem_ptr_s = reinterpret_cast<volatile uint32_t*>(smem + Smem::tmem_ptr);
   uint8_t* sUnits = smem + Smem::units;
 
   const int group = p.hq / p.hkv;
-  const int n_pairs = (group + 1) >> 1;
-  const int total_units = p.plan[0] * p.hkv * n_pairs;
+  const int total_units = p.plan[0] * p.hq;
   const int32_t* items = p.plan + 4;
   const int grid = gridDim.x, cta = blockIdx.x;
   const int n_rounds = (total_units + grid - 1) / grid;
   auto pos_of = [&](int k) { return k * grid + ((k & 1) ? grid - 1 - cta : cta); };
 
   // ---------------------------------------------------------------- one-time setup
-  for (int k = tid; k < kMaxUnitsSmem && k < n_rounds; k += (int)blockDim.x) {
+  for (int k = tid; k < kMaxUnitsSmem && k < n_rounds; k += kThreads) {
     const int pos = pos_of(k);
     Unit u;
     u.n_tiles = -1;
-    if (pos < total_units) u = get_unit(pos, p.hkv, group, items, p.seq_lens, p.cu_q);
+    if (pos < total_units) u = get_unit(pos, p.hq, group, items, p.seq_lens, p.cu_q);
     *reinterpret_cast<Unit*>(sUnits + k * 48) = u;
   }
   auto unit_at = [&](int k) {
@@ -177,23 +144,18 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     const int pos = pos_of(k);
     Unit u;
     u.n_tiles = -1;
-    if (pos < total_units) u = get_unit(pos, p.hkv, group, items, p.seq_lens, p.cu_q);
+    if (pos < total_units) u = get_unit(pos, p.hq, group, items, p.seq_lens, p.cu_q);
     return u;
   };
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(bar(kFullK + s), 1);
-      mbar_init(bar(kEmptyK + s), 1);
+      mbar_init(bar(kEmptyK + s), 8);  // one elected arrival per consumer warp
       mbar_init(bar(kFullV + s), 1);
-      mbar_init(bar(kEmptyV + s), 1);
+      mbar_init(bar(kEmptyV + s), 8);
     }
     mbar_init(bar(kQFull), 1);
-    mbar_init(bar(kQEmpty), 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar(kSFull + s), 1);
-      mbar_init(bar(kPFull + s), kFullRow ? 4 : 8);  // one elected arrival per softmax warp of the sub-tile
-      mbar_init(bar(kOFull + s), 1);
-    }
+    mbar_init(bar(kQEmpty), 8);
     fence_barrier_init();
     prefetch_tensormap(&map_q);
     prefetch_tensormap(&map_k);
@@ -205,18 +167,13 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     prefetch_tensormap(&newbox_k);
     prefetch_tensormap(&newbox_v);
   }
-  if (warp == 2) tmem_alloc(sbase + Smem::tmem_ptr, kTmemCols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_s;
 
-  // Register budget (full-row variant): the control warpgroup gives registers up, the softmax warpgroups take
-  // them.  Each setmaxnreg sits at the top of its own branch so that ptxas allocates per role.  The pool is what
-  // the CTA was launched with (384 threads x 168 registers = 64 512, NOT the 65 536 of the SM): 128 x 72 +
-  // 256 x 208 = 62 464 fits; a request beyond the pool would block in setmaxnreg.inc forever.
+  // Register budget: the producer warpgroup gives registers up, the consumer warpgroups take them.  Each
+  // setmaxnreg sits at the top of its own branch so that ptxas allocates per role.  The pool is what the CTA
+  // was launched with (384 threads x 168 registers = 64 512): 128 x 40 + 256 x 232 = 64 512.
   if (warp < 4) {
-   if constexpr (kFullRow) asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
+   asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
    if (warp < 2) {
     // ============================================================ TMA producers: warp 0 = K (+Q), warp 1 = V
     const int kind = warp;
@@ -229,7 +186,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     // ---- fused KV append: the tile of a unit that holds the unit's own new tokens is written to the
     // pool straight from shared memory (TMA store) when its ring slot is recycled -- no extra loads,
     // no extra launch.  Ownership: positions [cached + q_start, cached + min(q_len, q_start + 128)) of
-    // kv head h belong to the unit of query tile q_start and the first head pair.
+    // kv head h belong to the unit of query tile q_start and the first query head of the group.
     struct Pending {
       int valid, lo, hi, tile_begin, col0;
       uint32_t phase;
@@ -237,7 +194,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     } pend[kStages];
     for (int s = 0; s < kStages; ++s) pend[s].valid = 0;
     const CUtensorMap* smap_box = bmap;   // pool, box_rows x 64 columns
-    const CUtensorMap* smap_row = gmap;   // pool, 1 x 64 columns (row-exact / scatter4)
+    const CUtensorMap* smap_row = gmap;   // pool, 1 x 64 columns (row-exact)
     // valid: 0 = nothing, 1 = tile issued (append once it has landed), 2 = stores issued
     auto issue_stores = [&](int stage) {  // whole warp; the tile has landed
       Pending& pd = pend[stage];
@@ -261,12 +218,11 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
         for (int it = 0; it < 2; ++it) {
           const int grp = (lane >> 1) + it * 16, half = lane & 1;
           const int pos0 = pd.tile_begin + grp * 4;
-          int rr[4];
 #pragma unroll
           for (int i = 0; i < 4; ++i)
-            rr[i] = (pos0 + i >= pd.lo && pos0 + i < pd.hi) ? __ldg(pd.slots + pos0 + i) : p.num_slots;  // out of range: skipped
-          if (pos0 + 4 > pd.lo && pos0 < pd.hi)
-            tma_scatter4(smap_row, base + half * kHalfBytes + grp * 512, pd.col0 + half * 64, rr[0], rr[1], rr[2], rr[3]);
+            if (pos0 + i >= pd.lo && pos0 + i < pd.hi)
+              tma_store_2d(smap_row, base + half * kHalfBytes + (grp * 4 + i) * 128, pd.col0 + half * 64,
+                           __ldg(pd.slots + pos0 + i));
         }
       }
       bulk_commit();
@@ -290,27 +246,26 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
       if (u.n_tiles <= 0) continue;
       const int32_t* slots = p.slot_table + (int64_t)u.r * p.st_stride;
       const int col0 = u.h * kD;
-      const bool owner = !p.skip_append && (u.head0 == u.h * group);
+      const bool owner = !p.skip_append && u.owner;
       const int own_lo = u.cached + u.q_start, own_hi = u.cached + min(u.q_len, u.q_start + kBM);
-      // The unit's query sub-tiles are requested right AFTER its first K tile (see the tile loop): the Q
+      // The unit's query tile is requested right AFTER its first K tile (see the tile loop): the Q
       // buffer only becomes free once the previous unit's last QK^T has completed, whereas a K ring slot is
-      // usually free earlier -- so the first K tile of the next unit no longer queues behind the Q wait.
+      // usually free earlier -- so the first K tile of the next unit does not queue behind the Q wait.
       auto load_q = [&]() {
         // rows past the tensor end are zero filled, rows past the request's end belong to the next
         // request: computed, never stored
         mbar_wait(bar(kQEmpty), (unit_count & 1) ^ 1);
         if (lane == 0) {
-          mbar_arrive_expect_tx(bar(kQFull), (uint32_t)u.n_sub * kTileBytes);
-          for (int s = 0; s < u.n_sub; ++s)
-            for (int half = 0; half < 2; ++half)
-              tma_load_2d(sbase + Smem::q + s * kTileBytes + half * kHalfBytes, &map_q, bar(kQFull),
-                          (u.head0 + s) * kD + half * 64, u.q_begin + u.q_start);
+          mbar_arrive_expect_tx(bar(kQFull), (uint32_t)kTileBytes);
+          for (int half = 0; half < 2; ++half)
+            tma_load_2d(sbase + Smem::q + half * kHalfBytes, &map_q, bar(kQFull), u.head * kD + half * 64,
+                        u.q_begin + u.q_start);
         }
         __syncwarp();
       };
       // Positions < cached come from the pool through the slot table; positions >= cached are the
       // tokens of this very forward and are read straight from the k / v inputs (row q_begin + pos -
-      // cached), so the attention never depends on the append that warp 3 performs concurrently.
+      // cached), so the attention never depends on the append performed concurrently.
       // Rows past the end of the request are other requests' tokens or out of range (zeros): finite,
       // and masked by position.
       const CUtensorMap* nmap = kind == 0 ? &new_k : &new_v;
@@ -345,7 +300,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
             else load_rows_one_by_one(dst, fb, col, pb, rb);  // the box straddling cached_len
           }
         } else {
-          // gather mode: 32 row groups x 2 halves = 2 groups per lane
+          // row mode: 32 row groups of four x 2 halves = 2 groups per lane, one single-row box per row
           mbar_wait(bar(empty0 + stage), phase ^ 1);
           flush_stage(stage);
           if (lane == 0) mbar_arrive_expect_tx(bar(full0 + stage), kTileBytes);
@@ -359,10 +314,10 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
             const int col = col0 + half * 64;
             if (pos0 + 4 <= u.cached) {
               const int4 rr = __ldg(reinterpret_cast<const int4*>(slots + pos0));
-              tma_gather4(dst, gmap, fb, col, rr.x, rr.y, rr.z, rr.w);
-            } else if (pos0 >= u.cached) {
-              const int r0 = u.q_begin + pos0 - u.cached;
-              tma_gather4(dst, nmap, fb, col, r0, r0 + 1, r0 + 2, r0 + 3);
+              tma_load_2d(dst, gmap, fb, col, rr.x);
+              tma_load_2d(dst + 128, gmap, fb, col, rr.y);
+              tma_load_2d(dst + 256, gmap, fb, col, rr.z);
+              tma_load_2d(dst + 384, gmap, fb, col, rr.w);
             } else {
               load_rows_one_by_one(dst, fb, col, pos0, 4);
             }
@@ -393,397 +348,142 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
         issue_stores(s);
       }
     bulk_wait0();
-  } else if (warp == 2) {
-    // ============================================================ UMMA issuer (one thread)
-    if (lane == 0) {
-      constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, 128, kBf16, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, 128, kBf16, false, true);  // B = V, MN-major
-      uint32_t tile_count = 0, unit_count = 0;
-      uint32_t p_count[2] = {0, 0};  // P tiles consumed per sub-tile (phase of kPFull)
-      auto qk = [&](int s, uint32_t tc) {
-        const uint32_t kb = sbase + Smem::kring + (tc % kStages) * kTileBytes;
-        const uint32_t qa = sbase + Smem::q + s * kTileBytes;
-        const uint32_t d = tmem_base + s * 128;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint64_t da = make_smem_desc(qa + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
-          const uint64_t db = make_smem_desc(kb + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
-          umma_f16_ss(d, da, db, idesc_qk, kk > 0);
-        }
-        umma_commit(bar(kSFull + s));
-      };
-      auto pv = [&](int s, uint32_t tc, bool first) {
-        mbar_wait(bar(kPFull + s), p_count[s] & 1);
-        ++p_count[s];
-        tc_fence_after_sync();
-        const uint32_t vb = sbase + Smem::vring + (tc % kStages) * kTileBytes;
-        const uint32_t pa = tmem_base + s * 128;          // packed bf16 P over the S columns
-        const uint32_t d = tmem_base + 256 + s * 128;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          // B = V (MN-major): 16 keys = two 8-key swizzle atoms (1024 B each); dims 64..127 at +16 KB
-          const uint64_t db = make_smem_desc(vb + kk * 2048, kHalfBytes, 1024, kLayoutSW128);
-          // P (packed 16-bit pairs over the S columns).  full-row softmax: keys 0-127 in columns 0-63;
-          // half-row softmax: keys 0-63 in columns 0-31, keys 64-127 in columns 64-95 of the sub-tile
-          const uint32_t pcol = kFullRow ? (uint32_t)kk * 8 : (uint32_t)((kk >> 2) * 64 + (kk & 3) * 8);
-          umma_f16_ts(d, pa + pcol, db, idesc_pv, (!first) || kk > 0);
-        }
-        umma_commit(bar(kOFull + s));
-      };
-      for (int k = 0; k < n_rounds; ++k) {
-        const Unit u = unit_at(k);
-        if (u.n_tiles <= 0) continue;
-        mbar_wait(bar(kQFull), unit_count & 1);
-        ++unit_count;
-        // tile 0: scores of both sub-tiles
-        mbar_wait(bar(kFullK + tile_count % kStages), (tile_count / kStages) & 1);
-        tc_fence_after_sync();
-        for (int s = 0; s < u.n_sub; ++s) qk(s, tile_count);
-        umma_commit(bar(kEmptyK + tile_count % kStages));
-        if (u.n_tiles == 1) umma_commit(bar(kQEmpty));
-        for (int j = 0; j < u.n_tiles; ++j) {
-          const uint32_t tc = tile_count + j;
-          const bool more = j + 1 < u.n_tiles;
-          mbar_wait(bar(kFullV + tc % kStages), (tc / kStages) & 1);
-          if (more) mbar_wait(bar(kFullK + (tc + 1) % kStages), ((tc + 1) / kStages) & 1);
-          tc_fence_after_sync();
-          for (int s = 0; s < u.n_sub; ++s) {
-            pv(s, tc, j == 0);
-            if (more) qk(s, tc + 1);
-          }
-          umma_commit(bar(kEmptyV + tc % kStages));
-          if (more) {
-            umma_commit(bar(kEmptyK + (tc + 1) % kStages));
-            if (j + 2 == u.n_tiles) umma_commit(bar(kQEmpty));  // last QK of the unit issued
-          }
-        }
-        tile_count += u.n_tiles;
-      }
-    }
    }
-  } else if (kFullRow) {
-    // ============================================================ softmax: 8 warps, one thread per query row.
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-    // sub-tile A: warps 4-7, B: warps 8-11; warp & 3 = TMEM lane quadrant.
-    const int sub = (warp - 4) >> 2;
-    const int row = (warp & 3) * 32 + lane;         // query row of the sub-tile = TMEM lane
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    const uint32_t s_addr = tmem_base + lane_base + sub * 128;        // my 128 score columns
-    const uint32_t o_addr = tmem_base + lane_base + 256 + sub * 128;  // my 128 output columns
-    uint32_t my_tiles = 0;  // tiles this warpgroup processed (barrier phases)
-    for (int k = 0; k < n_rounds; ++k) {
-      const Unit u = unit_at(k);
-      if (u.n_tiles <= 0) continue;
-      if (sub >= u.n_sub) continue;  // odd group size: the B warpgroup sits this unit out
-      const int q_row = u.q_start + row;
-      const int vis_end = min(u.cached + q_row + 1, u.kv_len);  // keys [0, vis_end) are visible
-      float m_used = -INFINITY, l_run = 0.f;
-      for (int j = 0; j < u.n_tiles; ++j, ++my_tiles) {
-        const int tile_begin = j * kBN;
-        mbar_wait(bar(kSFull + sub), my_tiles & 1);
-        tc_fence_after_sync();
-        // visible keys of this row inside the tile form a prefix [0, n_vis); rows of a warp are consecutive,
-        // so lane 0 / lane 31 bound the warp: whole 32-column chunks are skipped, unmasked, or (at most two)
-        // masked element-wise -- warp-uniform branches
-        const int n_vis = max(0, min(kBN, vis_end - tile_begin));
-        const int n_lo = __shfl_sync(0xffffffffu, n_vis, 0), n_hi = __shfl_sync(0xffffffffu, n_vis, 31);
-        uint32_t s[128];
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (c * 32 < n_hi) tmem_ld32(s_addr + c * 32, s + c * 32);
-        tmem_wait_ld();
-        // ---- row max
-        float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int col0 = c * 32;
-          if (col0 >= n_hi) continue;
-          if (col0 + 32 <= n_lo) {
-#pragma unroll
-            for (int e = 0; e < 32; e += 4) {
-              mx0 = fmaxf(mx0, __uint_as_float(s[col0 + e]));
-              mx1 = fmaxf(mx1, __uint_as_float(s[col0 + e + 1]));
-              mx2 = fmaxf(mx2, __uint_as_float(s[col0 + e + 2]));
-              mx3 = fmaxf(mx3, __uint_as_float(s[col0 + e + 3]));
-            }
-          } else {
-            const int nv = n_vis - col0;
-#pragma unroll
-            for (int e = 0; e < 32; e += 4) {
-              mx0 = fmaxf(mx0, e < nv ? __uint_as_float(s[col0 + e]) : -INFINITY);
-              mx1 = fmaxf(mx1, e + 1 < nv ? __uint_as_float(s[col0 + e + 1]) : -INFINITY);
-              mx2 = fmaxf(mx2, e + 2 < nv ? __uint_as_float(s[col0 + e + 2]) : -INFINITY);
-              mx3 = fmaxf(mx3, e + 3 < nv ? __uint_as_float(s[col0 + e + 3]) : -INFINITY);
-            }
-          }
-        }
-        const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * p.scale_log2;
-        // ---- the previous PV of this sub-tile has completed (in-order tensor pipe); observe it so that the
-        // phase of kOFull never runs ahead of us, then rescale O if the max moved a lot (lazy correction)
-        if (j > 0) {
-          mbar_wait(bar(kOFull + sub), (my_tiles - 1) & 1);
-          tc_fence_after_sync();
-        }
-        const bool grow = mx > m_used + kRescaleThreshold;   // also true for the first tile (-inf)
-        const float m_new = grow ? mx : m_used;
-        if (j > 0 && __any_sync(0xffffffffu, grow)) {
-          const float alpha = grow ? fast_exp2(m_used - m_new) : 1.f;
-          l_run *= alpha;
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[32];
-            tmem_ld_x32(o_addr + c * 32, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int e = 0; e < 32; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-            tmem_st_x32(o_addr + c * 32, o);
-          }
-          tmem_wait_st();
-        }
-        m_used = m_new;
-        const float m_sub = (m_used == -INFINITY) ? 0.f : m_used;
-        // ---- P = exp2(S*scale - m), row sum, packed 16-bit pairs back to TMEM over my own S columns 0-63
-        float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int col0 = c * 32;
-          uint32_t pk[16];
-          if (col0 >= n_hi) {
-#pragma unroll
-            for (int e = 0; e < 16; ++e) pk[e] = 0u;
-          } else if (col0 + 32 <= n_lo) {
-#pragma unroll
-            for (int e = 0; e < 32; e += 2) {
-              const float p0 = fast_exp2(fmaf(__uint_as_float(s[col0 + e]), p.scale_log2, -m_sub));
-              const float p1 = fast_exp2(fmaf(__uint_as_float(s[col0 + e + 1]), p.scale_log2, -m_sub));
-              l0 += p0;
-              l1 += p1;
-              pk[e >> 1] = pack2<T>(p0, p1);
-            }
-          } else {
-            const int nv = n_vis - col0;
-#pragma unroll
-            for (int e = 0; e < 32; e += 2) {
-              const float p0 = e < nv ? fast_exp2(fmaf(__uint_as_float(s[col0 + e]), p.scale_log2, -m_sub)) : 0.f;
-              const float p1 = e + 1 < nv ? fast_exp2(fmaf(__uint_as_float(s[col0 + e + 1]), p.scale_log2, -m_sub)) : 0.f;
-              l0 += p0;
-              l1 += p1;
-              pk[e >> 1] = pack2<T>(p0, p1);
-            }
-          }
-          tmem_st_x16(s_addr + c * 16, pk);
-        }
-        l_run += l0 + l1;
-        tmem_wait_st();
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(kPFull + sub));  // every lane's P is in TMEM (wait::st + fence above)
-      }
-      // ---- epilogue: O / l -> out (my row, 128 columns = 256 contiguous bytes)
-      mbar_wait(bar(kOFull + sub), (my_tiles - 1) & 1);
-      tc_fence_after_sync();
-      const float inv = 1.f / l_run;
-      const bool store = q_row < u.q_len;
-      T* orow = p.out + ((int64_t)(u.q_begin + q_row) * p.hq + (u.head0 + sub)) * kD;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t o[32];
-        tmem_ld_x32(o_addr + c * 32, o);
-        tmem_wait_ld();
-        if (store) {
-#pragma unroll
-          for (int v4 = 0; v4 < 4; ++v4) {
-            Vec8 w;
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-              w.w[e] = pack2<T>(__uint_as_float(o[v4 * 8 + 2 * e]) * inv, __uint_as_float(o[v4 * 8 + 2 * e + 1]) * inv);
-            *reinterpret_cast<Vec8*>(orow + c * 32 + v4 * 8) = w;
-          }
-        }
-      }
-      // my O / S reads are complete (tmem_wait_ld); the next unit's PV(0) that overwrites O is gated on
-      // kPFull, which every warp of this warpgroup arrives on only after all its lanes finished the epilogue
-      tc_fence_before_sync();
-      __syncwarp();
-    }
   } else {
-    // ============================================================ softmax: 16 warps.
-    // sub-tile A: warps 4-7 (score columns 0-63) + 12-15 (columns 64-127); B: warps 8-11 + 16-19.
-    // Two threads share a query row (same TMEM lane, different column halves) and exchange only the
-    // per-tile row max through smem; row sums stay per thread until the epilogue.
-    const int sw = warp - 4;
-    const int sub = (sw >> 2) & 1;
-    const int half = sw >> 3;
-    const int row = (warp & 3) * 32 + lane;         // query row of the sub-tile = TMEM lane
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    const uint32_t s_addr = tmem_base + lane_base + sub * 128 + half * 64;        // my 64 score columns
-    const uint32_t o_addr = tmem_base + lane_base + 256 + sub * 128 + half * 64;  // my 64 output columns
-    float* red = reinterpret_cast<float*>(smem + Smem::red);  // [2 parity][2 sub][2 half][128]
-    uint32_t tile_count = 0, my_tiles = 0;          // my_tiles: tiles this warpgroup processed (phases)
+    // ============================================================ consumer warpgroups (64 query rows each)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    T* const tsel = nullptr;              // selects the bf16 / fp16 wgmma overload
+    const int wg = (warp - 4) >> 2;       // rows wg*64 .. wg*64+63 of the unit's query tile
+    const int cw = warp & 3;
+    // accumulator fragment (see sm90.cuh): rows ra = 16*cw + lane/4 and ra + 8 of the warpgroup's 64,
+    // columns 8i + 2*(lane%4) (+1), i = 0..15
+    const int ra = wg * 64 + 16 * cw + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    uint32_t tile_count = 0, unit_count = 0;
     for (int k = 0; k < n_rounds; ++k) {
       const Unit u = unit_at(k);
       if (u.n_tiles <= 0) continue;
-      if (sub >= u.n_sub) {  // odd group size: the B warpgroup sits this unit out
-        tile_count += u.n_tiles;
-        continue;
-      }
-      const int q_row = u.q_start + row;            // row within the request's new tokens
-      const int vis_end = min(u.cached + q_row + 1, u.kv_len);  // keys [0, vis_end) are visible
-      float m_used = -INFINITY, l_run = 0.f;
-      for (int j = 0; j < u.n_tiles; ++j, ++my_tiles) {
+      // keys [0, vis_end) are visible to a query row; the warpgroup's last row bounds the tiles it needs
+      const int vis0 = min(u.cached + u.q_start + ra + 1, u.kv_len);
+      const int vis1 = min(u.cached + u.q_start + ra + 9, u.kv_len);
+      const int wg_vis = min(u.cached + u.q_start + wg * 64 + 64, u.kv_len);
+      float o[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) o[i] = 0.f;
+      float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+      mbar_wait(bar(kQFull), unit_count & 1);
+      ++unit_count;
+      const uint32_t qa = sbase + Smem::q + wg * 8192;  // 64 rows x 128 B into each half
+      for (int j = 0; j < u.n_tiles; ++j, ++tile_count) {
+        const uint32_t stage = tile_count % kStages, phase = (tile_count / kStages) & 1;
         const int tile_begin = j * kBN;
-        mbar_wait(bar(kSFull + sub), my_tiles & 1);
-        tc_fence_after_sync();
-        // visible keys of this row inside the tile form a prefix [0, n_vis); rows of a warp are
-        // consecutive, so lane 0 / lane 31 bound the warp: whole 32-column chunks are either
-        // skipped, unmasked, or (at most two of them) masked element-wise -- warp-uniform branches
-        const int n_vis = max(0, min(kBN, vis_end - tile_begin));
-        const int n_lo = __shfl_sync(0xffffffffu, n_vis, 0), n_hi = __shfl_sync(0xffffffffu, n_vis, 31);
-        // ---- pass 1: row max over my 64 columns
-        float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
+        const bool active = tile_begin < wg_vis;  // warpgroup-uniform
+        mbar_wait(bar(kFullK + stage), phase);
+        float s[64];
+        if (active) {
+          const uint32_t kb = sbase + Smem::kring + stage * kTileBytes;
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int col0 = half * 64 + c * 32;
-          if (col0 >= n_hi) continue;  // every row of this warp has the chunk masked
-          uint32_t s[32];
-          tmem_ld_x32(s_addr + c * 32, s);
-          tmem_wait_ld();
-          if (col0 + 32 <= n_lo) {
+          for (int i = 0; i < 64; ++i) s[i] = 0.f;
+          wgmma_fence();
 #pragma unroll
-            for (int e = 0; e < 32; e += 4) {
-              mx0 = fmaxf(mx0, __uint_as_float(s[e]));
-              mx1 = fmaxf(mx1, __uint_as_float(s[e + 1]));
-              mx2 = fmaxf(mx2, __uint_as_float(s[e + 2]));
-              mx3 = fmaxf(mx3, __uint_as_float(s[e + 3]));
-            }
-          } else {
-            const int nv = n_vis - col0;
-#pragma unroll
-            for (int e = 0; e < 32; e += 4) {
-              mx0 = fmaxf(mx0, e < nv ? __uint_as_float(s[e]) : -INFINITY);
-              mx1 = fmaxf(mx1, e + 1 < nv ? __uint_as_float(s[e + 1]) : -INFINITY);
-              mx2 = fmaxf(mx2, e + 2 < nv ? __uint_as_float(s[e + 2]) : -INFINITY);
-              mx3 = fmaxf(mx3, e + 3 < nv ? __uint_as_float(s[e + 3]) : -INFINITY);
-            }
+          for (int kk = 0; kk < 8; ++kk) {
+            const uint64_t da = make_smem_desc(qa + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
+            const uint64_t db = make_smem_desc(kb + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
+            wgmma_m64n128k16_ss(s, da, db, kk > 0, tsel);
           }
+          wgmma_commit();
+          wgmma_wait0();
         }
-        float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-        // exchange with the thread holding the other half of the row
-        float* rp = red + ((my_tiles & 1) * 4 + sub * 2) * 128;
-        rp[half * 128 + row] = mx;
-        named_bar_sync(1 + sub, 256);
-        mx = fmaxf(mx, rp[(half ^ 1) * 128 + row]) * p.scale_log2;
-        // ---- the previous PV of this sub-tile has completed (in-order tensor pipe); observe it so
-        // that the phase of kOFull never runs ahead of us, then rescale O if the max moved a lot
-        if (j > 0) {
-          mbar_wait(bar(kOFull + sub), (my_tiles - 1) & 1);
-          tc_fence_after_sync();
-        }
-        const bool grow = mx > m_used + kRescaleThreshold;   // also true for the first tile (-inf)
-        const float m_new = grow ? mx : m_used;
-        if (j > 0 && __any_sync(0xffffffffu, grow)) {
-          const float alpha = grow ? fast_exp2(m_used - m_new) : 1.f;
-          l_run *= alpha;
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t o[32];
-            tmem_ld_x32(o_addr + c * 32, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int e = 0; e < 32; ++e) o[e] = __float_as_uint(__uint_as_float(o[e]) * alpha);
-            tmem_st_x32(o_addr + c * 32, o);
-          }
-          tmem_wait_st();
-        }
-        m_used = m_new;
-        const float m_sub = (m_used == -INFINITY) ? 0.f : m_used;
-        // ---- pass 2: P = exp2(S*scale - m), row sum, packed bf16 back to TMEM over my own S
-        // columns (keys 0-63 -> columns 0-31, keys 64-127 -> columns 64-95 of the sub-tile)
-        float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int col0 = half * 64 + c * 32;
-          uint32_t pk[16];
-          if (col0 >= n_hi) {
-#pragma unroll
-            for (int e = 0; e < 16; ++e) pk[e] = 0u;
-          } else {
-            uint32_t s[32];
-            tmem_ld_x32(s_addr + c * 32, s);
-            tmem_wait_ld();
-            if (col0 + 32 <= n_lo) {
-#pragma unroll
-              for (int e = 0; e < 32; e += 2) {
-                const float p0 = fast_exp2(fmaf(__uint_as_float(s[e]), p.scale_log2, -m_sub));
-                const float p1 = fast_exp2(fmaf(__uint_as_float(s[e + 1]), p.scale_log2, -m_sub));
-                l0 += p0;
-                l1 += p1;
-                pk[e >> 1] = pack2<T>(p0, p1);
-              }
-            } else {
-              const int nv = n_vis - col0;
-#pragma unroll
-              for (int e = 0; e < 32; e += 2) {
-                const float p0 = e < nv ? fast_exp2(fmaf(__uint_as_float(s[e]), p.scale_log2, -m_sub)) : 0.f;
-                const float p1 = e + 1 < nv ? fast_exp2(fmaf(__uint_as_float(s[e + 1]), p.scale_log2, -m_sub)) : 0.f;
-                l0 += p0;
-                l1 += p1;
-                pk[e >> 1] = pack2<T>(p0, p1);
-              }
-            }
-          }
-          tmem_st_x16(s_addr + c * 16, pk);
-        }
-        l_run += l0 + l1;
-        tmem_wait_st();
-        tc_fence_before_sync();
         __syncwarp();
-        if (lane == 0) mbar_arrive(bar(kPFull + sub));  // every lane's P is in TMEM (wait::st + fence above)
-      }
-      // ---- epilogue: O / l -> out (my 64 output columns); l = sum of the two half-row sums
-      float* lp = red + (2 * 4 + sub * 2) * 128;  // third buffer, after the two parity buffers
-      lp[half * 128 + row] = l_run;
-      mbar_wait(bar(kOFull + sub), (my_tiles - 1) & 1);
-      tc_fence_after_sync();
-      named_bar_sync(1 + sub, 256);
-      const float inv = 1.f / (l_run + lp[(half ^ 1) * 128 + row]);
-      const bool store = q_row < u.q_len;
-      T* orow = p.out + ((int64_t)(u.q_begin + q_row) * p.hq + (u.head0 + sub)) * kD + half * 64;
+        if (lane == 0) {
+          mbar_arrive(bar(kEmptyK + stage));
+          if (j + 1 == u.n_tiles) mbar_arrive(bar(kQEmpty));  // last QK of the unit
+        }
+        uint32_t pa[8][4];
+        if (active) {
+          // ---- scale, causal mask, online softmax (a row's 128 columns live in one quad of lanes)
+          float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t o[32];
-        tmem_ld_x32(o_addr + c * 32, o);
-        tmem_wait_ld();
-        if (store) {
+          for (int i = 0; i < 16; ++i)
 #pragma unroll
-          for (int v4 = 0; v4 < 4; ++v4) {
-            Vec8 w;
+            for (int x = 0; x < 4; ++x) {
+              const int key = tile_begin + 8 * i + cq + (x & 1);
+              const float v = key < ((x >> 1) ? vis1 : vis0) ? s[4 * i + x] * p.scale_log2 : -INFINITY;
+              s[4 * i + x] = v;
+              mx[x >> 1] = fmaxf(mx[x >> 1], v);
+            }
+          float alpha[2], m_use[2];
 #pragma unroll
-            for (int e = 0; e < 4; ++e)
-              w.w[e] = pack2<T>(__uint_as_float(o[v4 * 8 + 2 * e]) * inv, __uint_as_float(o[v4 * 8 + 2 * e + 1]) * inv);
-            *reinterpret_cast<Vec8*>(orow + c * 32 + v4 * 8) = w;
+          for (int e = 0; e < 2; ++e) {
+            mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 1));
+            mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 2));
+            const float m_new = fmaxf(m_run[e], mx[e]);
+            m_use[e] = (m_new == -INFINITY) ? 0.f : m_new;
+            alpha[e] = fast_exp2(m_run[e] - m_use[e]);
+            m_run[e] = m_new;
+          }
+          float ps[2] = {0.f, 0.f};
+#pragma unroll
+          for (int i = 0; i < 64; ++i) {
+            const float e = fast_exp2(s[i] - m_use[(i >> 1) & 1]);
+            s[i] = e;
+            ps[(i >> 1) & 1] += e;
+            o[i] *= alpha[(i >> 1) & 1];
+          }
+#pragma unroll
+          for (int e = 0; e < 2; ++e) l_run[e] = l_run[e] * alpha[e] + ps[e];
+          // P as the 16-bit A fragment of k-block kb (keys 16kb .. 16kb+15)
+#pragma unroll
+          for (int kb = 0; kb < 8; ++kb) {
+            pa[kb][0] = pack2<T>(s[8 * kb + 0], s[8 * kb + 1]);
+            pa[kb][1] = pack2<T>(s[8 * kb + 2], s[8 * kb + 3]);
+            pa[kb][2] = pack2<T>(s[8 * kb + 4], s[8 * kb + 5]);
+            pa[kb][3] = pack2<T>(s[8 * kb + 6], s[8 * kb + 7]);
           }
         }
+        mbar_wait(bar(kFullV + stage), phase);
+        if (active) {
+          const uint32_t vb = sbase + Smem::vring + stage * kTileBytes;
+          wgmma_fence();
+#pragma unroll
+          for (int kb = 0; kb < 8; ++kb) {
+            // B = V (MN-major): 16 keys = two 8-key swizzle atoms (1024 B each); dims 64..127 at +16 KB
+            const uint64_t db = make_smem_desc(vb + kb * 2048, kHalfBytes, 1024, kLayoutSW128);
+            wgmma_m64n128k16_rs(o, pa[kb], db, 1u, tsel);
+          }
+          wgmma_commit();
+          wgmma_wait0();
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar(kEmptyV + stage));
       }
-      tc_fence_before_sync();  // O / S of this sub-tile may be overwritten by the next unit's MMAs
-      named_bar_sync(1 + sub, 256);  // lp is reused by the next unit
-      tile_count += u.n_tiles;
+      // ---- epilogue: O / l -> out, rows ra and ra + 8 (row sums reduced over the quad)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        l_run[e] += __shfl_xor_sync(0xffffffffu, l_run[e], 1);
+        l_run[e] += __shfl_xor_sync(0xffffffffu, l_run[e], 2);
+      }
+      const float inv[2] = {1.f / l_run[0], 1.f / l_run[1]};
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int q_row = u.q_start + ra + 8 * e;
+        if (q_row < u.q_len) {
+          T* orow = p.out + ((int64_t)(u.q_begin + q_row) * p.hq + u.head) * kD + cq;
+#pragma unroll
+          for (int i = 0; i < 16; ++i)
+            *reinterpret_cast<uint32_t*>(orow + 8 * i) = pack2<T>(o[4 * i + 2 * e] * inv[e], o[4 * i + 2 * e + 1] * inv[e]);
+        }
+      }
     }
   }
 
   // ---------------------------------------------------------------- teardown
-  tc_fence_before_sync();
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 template <typename T>
 static int launch(const Params<T>& p, const void* q, int64_t q_rs, int64_t nnz, const void* k_cache,
-                  const void* v_cache, cudaStream_t st, bool full_row) {
+                  const void* v_cache, cudaStream_t st) {
   CUtensorMap nk, nv, nbk, nbv;
   const bool bf16 = std::is_same<T, __nv_bfloat16>::value;
   CUtensorMap mq, mk, mv, bk, bv;
@@ -810,16 +510,11 @@ static int launch(const Params<T>& p, const void* q, int64_t q_rs, int64_t nnz, 
   const size_t smem = Smem::total + 1024;
   static bool configured = false;
   if (!configured) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_tc_kernel<T, true>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_tc_kernel<T, false>,
+    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_tc_kernel<T>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  if (full_row)
-    attn_prefill_tc_kernel<T, true><<<num_sms(), kThreadsFullRow, smem, st>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
-  else
-    attn_prefill_tc_kernel<T, false><<<num_sms(), kThreadsHalfRow, smem, st>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
+  attn_prefill_tc_kernel<T><<<num_sms(), kThreads, smem, st>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
   B200_POST_LAUNCH();
   return 0;
 }
@@ -827,7 +522,6 @@ static int launch(const Params<T>& p, const void* q, int64_t q_rs, int64_t nnz, 
 }  // namespace ptc
 
 extern std::atomic<int> g_prefill_skip_append;
-extern std::atomic<int> g_prefill_full_row;
 
 // entry used by b200_attn_prefill (attn_prefill.cu)
 int launch_prefill_tc(const void* q, int64_t q_rs, int64_t nnz, const void* k, const void* v, int64_t kv_rs,
@@ -849,7 +543,7 @@ int launch_prefill_tc(const void* q, int64_t q_rs, int64_t nnz, const void* k, c
   ptc::Params<T_> p{slot_table, st_stride, seq_lens, cu_q, prefill_plan, bs, hq, hkv, (int)num_slots, \
                     box_rows, scale_log2, (T_*)out, (const T_*)k, (const T_*)v, kv_rs, (T_*)k_cache,  \
                     (T_*)v_cache, out_loc, nnz, g_prefill_skip_append.load()};                                                   \
-  return ptc::launch<T_>(p, q, q_rs, nnz, k_cache, v_cache, st, g_prefill_full_row.load() != 0)
+  return ptc::launch<T_>(p, q, q_rs, nnz, k_cache, v_cache, st)
   if (dtype == B200_DTYPE_BF16) {
     RUN(__nv_bfloat16);
   }

@@ -25,23 +25,16 @@ namespace b200 {
 std::atomic<int> g_use_pdl{1};
 std::atomic<int> g_decode_impl{1};
 std::atomic<int> g_prefill_impl{1};
-std::atomic<int> g_prefill_order{0};  // 0 = size-sorted + snake dealing (balanced; measured best), 1 = request-major
+std::atomic<int> g_prefill_order{0};  // 0 = size-sorted + snake dealing (balanced), 1 = request-major
 std::atomic<int> g_prefill_skip_append{0};  // debug only
-// 1 = one softmax thread per query row (8 warps, FA4 style), 0 = two (16 warps).  Measured on B200 (round 2,
-// gpurun_out/r2c4): cfg1 prompts 312 vs 340 TF/s, 2 x 4096-token GQA-8 prompts 678 vs 695 TF/s -> default 0.
-std::atomic<int> g_prefill_full_row{0};
-std::atomic<int> g_decode_lookahead{4};
-// Split-KV policy (measured, profiles/r01_decode_plan_sweep.json): splitting costs a partial (o, m, l)
-// round trip plus the combine pass, so it only pays when whole requests cannot fill the grid.
+// Split-KV policy: splitting costs a partial (o, m, l) round trip plus the combine pass, so it only pays
+// when whole requests cannot fill the grid.
 std::atomic<int> g_decode_plan_target{2};    // when splitting, aim at target * CTA-hint / kv_heads (request, chunk) items
 std::atomic<int> g_decode_plan_nosplit{75};  // no split once bs * kv_heads * 100 >= nosplit * CTA-hint (0 = always split)
 // 0 = separate combine launch, 1 = the last-arriving chunk's CTA merges the partials in the decode launch (no
-// combine launch at all), 2 = in-kernel exactly when the policy above does not split.  Measured in captured
-// graphs (profiles/r02_decode_merge_sweep.json, after the merge's loads were batched): 1 is faster or equal at every
-// batch / head shape but one (bs 4, hq 8: 11.1 vs 10.6 us); tp4 shard 164.8 k -> 170.1 k tok/s, tp8 shard 233 k -> 252 k.
+// combine launch at all), 2 = in-kernel exactly when the policy above does not split.
 std::atomic<int> g_decode_fused_combine{1};
 std::atomic<int> g_decode_early_kv{1};  // captured decode launches stream K/V without waiting for the predecessor
-std::atomic<int> g_decode_defer{1};  // unit epilogue deferred behind the next unit's first tile
 }
 
 extern "C" int b200_abi_version(void) { return 7; }
@@ -61,14 +54,11 @@ extern "C" int b200_set_option(const char* name, int value) {
   if (name != nullptr && std::strcmp(name, "use_pdl") == 0) return b200::g_use_pdl.exchange(value);
   if (name != nullptr && std::strcmp(name, "decode_impl") == 0) return b200::g_decode_impl.exchange(value);
   if (name != nullptr && std::strcmp(name, "prefill_skip_append") == 0) return b200::g_prefill_skip_append.exchange(value);
-  if (name != nullptr && std::strcmp(name, "prefill_full_row") == 0) return b200::g_prefill_full_row.exchange(value);
   if (name != nullptr && std::strcmp(name, "prefill_order") == 0) return b200::g_prefill_order.exchange(value);
   if (name != nullptr && std::strcmp(name, "prefill_impl") == 0) return b200::g_prefill_impl.exchange(value);
-  if (name != nullptr && std::strcmp(name, "decode_lookahead") == 0) return b200::g_decode_lookahead.exchange(value);
   if (name != nullptr && std::strcmp(name, "decode_plan_target") == 0) return b200::g_decode_plan_target.exchange(value);
   if (name != nullptr && std::strcmp(name, "decode_plan_nosplit") == 0) return b200::g_decode_plan_nosplit.exchange(value);
   if (name != nullptr && std::strcmp(name, "decode_early_kv") == 0) return b200::g_decode_early_kv.exchange(value);
-  if (name != nullptr && std::strcmp(name, "decode_defer_epilogue") == 0) return b200::g_decode_defer.exchange(value);
   if (name != nullptr && std::strcmp(name, "decode_fused_combine") == 0) return b200::g_decode_fused_combine.exchange(value);
   return -1;
 }
@@ -81,5 +71,5 @@ extern "C" int b200_device_supported(void) {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }

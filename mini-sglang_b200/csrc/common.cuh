@@ -1,4 +1,4 @@
-// Shared device/host helpers for the sm_100a kernels of libb200attn.
+// Shared device/host helpers for the sm_90a kernels of libb200attn.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -48,7 +48,7 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev);
-    if (cached <= 0) cached = 148;
+    if (cached <= 0) cached = 132;
   }
   return cached;
 }

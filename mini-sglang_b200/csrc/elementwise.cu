@@ -1,4 +1,4 @@
-// Memory-bound elementwise kernels of the attention path, sm_100a:
+// Memory-bound elementwise kernels of the attention path, sm_90a:
 //   K1 store_kv        (reference: python/minisgl/kernel/csrc/jit/store.cu:28-53)
 //   K7 rmsnorm / fused_add_rmsnorm (reference call sites python/minisgl/layers/norm.py:8-38)
 //   K6 rope_neox       (reference call site python/minisgl/layers/rotary.py:45-51)

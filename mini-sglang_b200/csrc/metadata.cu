@@ -295,9 +295,8 @@ extern "C" int b200_build_metadata(const int32_t* req_info, int bs, const int32_
   }
   const int ctas = num_ctas_hint > 0 ? num_ctas_hint : 2 * num_sms();
   // (request, chunk) items to aim at when splitting: g_decode_plan_target x CTA-hint / kv heads for the full
-  // model (8 kv heads per rank); TP shards (<= 4 kv heads per rank: every unit is short) do better with
-  // half as many, larger chunks (measured on the tp2/4/8 shard shapes, profiles/r02_decode_sweep_tp.json:
-  // up to -18% at bs 40, hkv 1)
+  // model (8 kv heads per rank); TP shards (<= 4 kv heads per rank: every unit is short) get half as many,
+  // larger chunks
   int tgt = g_decode_plan_target.load();
   if (num_kv_heads <= 4 && tgt > 1) tgt /= 2;
   int target = (ctas * tgt) / num_kv_heads;

@@ -2,7 +2,7 @@
 // the CUDA runtime, so libb200attn.so does not link against libcuda) and a small cache keyed by
 // (base pointer, shape) -- the KV pool layers are the only tensors ever described.
 #include "common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 #include <cudaTypedefs.h>
 

@@ -6,7 +6,7 @@ The reference routes every TP collective through ``DistributedCommunicator.plugi
 ``enable_pynccl_distributed`` (impl.py:71-90).  :func:`enable_b200_allreduce` appends
 :class:`B200DistributedImpl` the same way: decode-sized ``all_reduce`` calls (one per layer after
 ``o_proj`` and after ``down_proj``, layers/linear.py:102-106,122-126 -- inside the captured decode
-graphs) run the sm_100a push kernel of ``csrc/allreduce.cu``; larger messages (prefill) and
+graphs) run the sm_90a push kernel of ``csrc/allreduce.cu``; larger messages (prefill) and
 ``all_gather`` are handed to the plug-in that was active before (the reference's NCCL), as
 north_star keeps it.
 

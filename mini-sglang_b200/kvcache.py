@@ -3,7 +3,7 @@
 
 Inside mini-sglang the engine's own pool is borrowed as is (same layout); this class exists so the
 backend, the tests and ``bench.py`` can run where the reference is not installed, and so that
-``store_kv`` goes through the sm_100a store kernel.
+``store_kv`` goes through the sm_90a store kernel.
 
 HBM layout (identical to the reference): one tensor ``[2, L, num_pages, page_size, Hkv_local, D]``;
 ``k_cache(l)`` / ``v_cache(l)`` are the contiguous ``[num_pages, page_size, Hkv_local, D]`` slices;

@@ -1,5 +1,5 @@
 """The layers that feed attention, with the reference's class and method names
-(``python/minisgl/layers/norm.py``, ``rotary.py``, ``attention.py``), bound to the sm_100a kernels.
+(``python/minisgl/layers/norm.py``, ``rotary.py``, ``attention.py``), bound to the sm_90a kernels.
 
 Two ways to use them:
 
@@ -195,7 +195,7 @@ class AttentionLayer:
 
 def patch_minisgl_layers(model: Any) -> int:
     """Re-bind the kernel attributes of every reference norm / rotary layer found under ``model``
-    (any object graph of ``BaseOP``s) to the sm_100a ops.  Returns the number of re-bound layers."""
+    (any object graph of ``BaseOP``s) to the sm_90a ops.  Returns the number of re-bound layers."""
     seen, count = set(), 0
     stack = [model]
     while stack:
@@ -232,7 +232,7 @@ _FLASHINFER_SAVED: Dict[str, Callable] = {}
 
 def patch_flashinfer_entry_points() -> int:
     """Point ``flashinfer.rmsnorm`` / ``fused_add_rmsnorm`` / ``apply_rope_with_cos_sin_cache_inplace``
-    at the sm_100a ops.  The reference's layers import these names from the ``flashinfer`` package
+    at the sm_90a ops.  The reference's layers import these names from the ``flashinfer`` package
     inside ``__init__`` (layers/norm.py:10,25, layers/rotary.py:35), so calling this BEFORE the model is
     built (``LLM(...)`` / ``Engine(...)``) makes every norm / rotary layer bind our kernels -- including
     inside the decode CUDA graphs, which are captured during ``Engine.__init__`` (engine/engine.py:100,
@@ -252,8 +252,8 @@ def patch_flashinfer_entry_points() -> int:
 
 
 def install_into_minisgl(norm_rope: bool = True, row_gather: bool = True) -> bool:
-    """One call, before ``LLM(...)`` / ``Engine(...)``: makes the reference build its model with the sm_100a
-    norm / RoPE kernels and use the sm_100a row gather, with zero edits to the reference.
+    """One call, before ``LLM(...)`` / ``Engine(...)``: makes the reference build its model with the sm_90a
+    norm / RoPE kernels and use the sm_90a row gather, with zero edits to the reference.
 
     ``Engine.__init__`` asserts that CUDA is not initialised yet (engine/engine.py:31) and importing
     ``flashinfer`` initialises it, so the FlashInfer names cannot be re-bound up front.  Instead the module
@@ -288,7 +288,7 @@ def restore_flashinfer_entry_points() -> None:
 
 
 def patch_minisgl_kernels() -> bool:
-    """Point ``minisgl.kernel.indexing`` at the sm_100a row gather.  ``VocabParallelEmbedding.forward``
+    """Point ``minisgl.kernel.indexing`` at the sm_90a row gather.  ``VocabParallelEmbedding.forward``
     imports the function from ``minisgl.kernel`` at call time (reference layers/embedding.py:32-34),
     so re-binding the package attribute is enough; no reference edit.  Returns False when the
     reference package is not importable (nothing to patch)."""

@@ -1,5 +1,5 @@
 """Operator-level host API: the functions the reference's layers call, same names and argument
-meaning, backed by the sm_100a kernels through the C ABI.
+meaning, backed by the sm_90a kernels through the C ABI.
 
 =====================================================  =====================================
 reference call site                                     function here
@@ -36,7 +36,7 @@ def _require_cuda(*ts: torch.Tensor) -> None:
     for t in ts:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                "mini-sglang_b200 ops need CUDA tensors (sm_100a kernels; no CPU fallback)"
+                "mini-sglang_b200 ops need CUDA tensors (sm_90a kernels; no CPU fallback)"
             )
 
 

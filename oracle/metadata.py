@@ -84,7 +84,7 @@ def ref_indices_flat(page_table: np.ndarray, reqs: Sequence[ReqTriple]) -> np.nd
 
 def ref_slot_table(page_table: np.ndarray, reqs: Sequence[ReqTriple]) -> np.ndarray:
     """Token-granular snapshot ``page_table[table_idx, :max_k]`` (the page_size==1 case of
-    fa.py:92-94); this is the dialect the B200 kernels consume."""
+    fa.py:92-94); this is the dialect the project's kernels consume."""
     max_k = max(d for (_, _, d) in reqs)
     return np.stack([page_table[t, :max_k] for (t, _, _) in reqs]).astype(np.int32)
 

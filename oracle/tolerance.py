@@ -11,10 +11,10 @@ for bf16 logits and bit-exact for page-table / indexing".  Two comparisons occur
     (two correct implementations whose exact results agree to 1e-3 may still round an element to
     adjacent 16-bit values; ulp = 2^-7 |x| for bf16, 2^-10 |x| for fp16).
     The reported number is  max_i (|a_i - b_i| - ulp |b_i|)^+ / max|b|.  north_star's figure is 1e-3; the
-    reference's OWN two GPU paths (FlashInfer fa2 vs TRT-LLM-gen) measure 0.9e-3 .. 1.1e-3 against each other
-    under this very formula on the cfg1 decode shapes (bench.py ref_gpu.*parity_trtllm_vs_fi, B200, round 2):
-    16-bit P makes 1e-3 the noise floor of the method.  Gate: GPU_REL_TOL = 1.5e-3 (1e-3 + that spread's
-    headroom); bench.py prints the number and the reference-vs-reference number side by side.
+    reference's OWN two GPU paths (FlashInfer fa2 vs TRT-LLM-gen) differ from each other by about that much
+    under this very formula (bench.py reports ref_gpu.*parity_trtllm_vs_fi where both run): 16-bit P makes
+    1e-3 the noise floor of the method.  Gate: GPU_REL_TOL = 1.5e-3 (1e-3 + that spread's headroom);
+    bench.py prints the number and the reference-vs-reference number side by side.
 
 ``vs_exact_oracle(a, ref32)`` -- against the exact fp32 oracle (oracle/attention.py: no 16-bit P, no
     output rounding): the reference's own kernels differ from it by the P rounding (|dP/P| <= 2^-9,

@@ -1,4 +1,4 @@
-"""pytest configuration: `-m gpu` tests need a B200, everything else runs on CPU."""
+"""pytest configuration: `-m gpu` tests need an H100, everything else runs on CPU."""
 import importlib
 import sys
 from pathlib import Path
@@ -11,7 +11,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200, sm_100a)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a)")
     config.addinivalue_line("markers", "slow: long-running CPU test")
 
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Golden vectors for the FLOATING-POINT side of the boundary, produced on a B200 by calling
+"""Golden vectors for the FLOATING-POINT side of the boundary, produced on the GPU by calling
 FlashInfer exactly the way the reference's call sites do (the reference's arithmetic for this path
 lives in flashinfer-python, pinned >=0.5.3 in its pyproject.toml:30; 0.6.11.post2 in this image):
 
@@ -16,7 +16,7 @@ Run on the GPU box (JIT modules are pre-built by tools/flashinfer_prebuild.py):
 Writes gpurun_out/flashinfer_golden.npz (inputs + FlashInfer outputs, bf16 stored as uint16); the
 file is then committed as tests/golden/flashinfer_golden.npz and checked by
 tests/test_oracle_golden.py (oracle vs FlashInfer) -- and this script prints, for the record, how
-the B200 kernels compare with FlashInfer on the same inputs.
+the project's kernels compare with FlashInfer on the same inputs.
 """
 import importlib
 import os
@@ -102,7 +102,7 @@ def main():
         a, b = ours.float(), fi_out.float()
         err = (a - b).abs().max().item() / b.abs().max().item()
         fro = ((a - b).norm() / b.norm()).item()
-        report.append(f"{phase}: B200 kernel vs FlashInfer fa2: max|d|/max|ref| = {err:.2e}, rel_fro = {fro:.2e}")
+        report.append(f"{phase}: project kernel vs FlashInfer fa2: max|d|/max|ref| = {err:.2e}, rel_fro = {fro:.2e}")
         used = np.unique(np.concatenate([md.slot_table[i, : md.cache_seqlens[i]] for i in range(len(w.reqs))]))
         out[f"{phase}_reqs"] = np.array(w.reqs, dtype=np.int32)
         out[f"{phase}_page_table"] = w.page_table
@@ -128,7 +128,7 @@ def main():
     mine = x.to(dev)
     pkg.ops.apply_rope_with_cos_sin_cache_inplace(pos.to(dev), mine[:, : HQ * D], mine[:, HQ * D : (HQ + HKV) * D], D, cache.to(dev))
     out["rope_x"], out["rope_pos"], out["rope_out"] = u16(x), pos.numpy(), u16(xg)
-    report.append(f"rope: B200 vs FlashInfer bit-identical = {bool(torch.equal(mine.view(torch.int16), xg.view(torch.int16)))}, "
+    report.append(f"rope: project kernel vs FlashInfer bit-identical = {bool(torch.equal(mine.view(torch.int16), xg.view(torch.int16)))}, "
                   f"max |d| = {(mine.float() - xg.float()).abs().max().item():.3e}")
 
     # ---- RMSNorm (2-D), per-head (3-D, in place), fused add

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Golden outputs of the reference's TWO GPU attention paths at the BASELINE head shapes, produced on a
-B200 by calling FlashInfer exactly as the reference's backends do:
+"""Golden outputs of the reference's TWO GPU attention paths at the BASELINE head shapes, produced on the
+GPU by calling FlashInfer exactly as the reference's backends do:
 
   * "fi":     BatchDecode / BatchPrefillWithPagedKVCacheWrapper, backend "fa2", page_size-1 view
               (python/minisgl/attention/fi.py:93-103,134-165,185-188; use_tensor_cores = GQA >= 4, fi.py:235-241)

@@ -1,6 +1,6 @@
 """Multi-GPU parity of the one-shot NVLink all-reduce (csrc/allreduce.cu, SURVEY 8(f) rank 4): spawns
 tools/ar_check.py under torch.distributed.run with 2 ranks (needs >= 2 GPUs; skipped on a 1-GPU box --
-run `gpurun --gpus 2 -- python -m pytest tests/test_gpu_allreduce.py -m gpu`).  The checks themselves
+run `python -m pytest tests/test_gpu_allreduce.py -m gpu` on a machine with two).  The checks themselves
 (bit-exact rank-order fp32 sum, identical bits on all ranks, == NCCL at world 2, fused residual +
 RMSNorm == unfused sequence, CUDA-graph replay, 1500-call stress, the reference's plug-in point) are
 documented in tools/ar_check.py."""

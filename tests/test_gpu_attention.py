@@ -1,5 +1,5 @@
 """GPU parity: metadata, decode / prefill attention with fused append, CUDA-graph hooks --
-product path (B200AttnBackend -> C ABI -> sm_100a kernels) vs the CPU oracle."""
+product path (B200AttnBackend -> C ABI -> sm_90a kernels) vs the CPU oracle."""
 import random
 
 import numpy as np
@@ -14,21 +14,19 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(params=[1, 0, 2, 3], ids=["tcgen05", "cpasync", "tcgen05-inorder-combine-launch", "tcgen05-combine-auto"])
 def decode_impl(request, b200, native_lib):
-    """Both decode kernels are held to the same oracle: the tcgen05 + TMA product kernel (with the
-    unit epilogue deferred behind the next unit's first tile -- the default -- and strictly in
-    order; with the split-KV merge done by the last-arriving chunk inside the decode launch -- the
-    default --, as its own launch, and under the "in kernel only when nothing is split" policy) and the
-    cp.async / CUDA-core bring-up kernel (selected with the debug options)."""
+    """Both decode kernels are held to the same oracle: the tensor-core + TMA product kernel (wgmma on
+    sm_90a; the ids keep the variant names the suite has always used) with the split-KV merge done by
+    the last-arriving chunk inside the decode launch -- the default --, as its own launch, and under
+    the "in kernel only when nothing is split" policy, and the cp.async / CUDA-core bring-up kernel
+    (selected with the debug options)."""
     impl = 0 if request.param == 0 else 1
     try:
         prev = b200._cabi.set_option("decode_impl", impl)
     except b200._cabi.B200NativeError:
         pytest.skip("cross-check kernel not in this build (B200_BUILD_BRINGUP=1)")
-    prev_defer = b200._cabi.set_option("decode_defer_epilogue", 0 if request.param == 2 else 1)
     prev_merge = b200._cabi.set_option("decode_fused_combine", {3: 2, 2: 0}.get(request.param, 1))
     yield impl
     b200._cabi.set_option("decode_impl", prev)
-    b200._cabi.set_option("decode_defer_epilogue", prev_defer)
     b200._cabi.set_option("decode_fused_combine", prev_merge)
 
 
@@ -149,16 +147,17 @@ def test_decode_second_layer_of_pool(b200, native_lib, decode_impl):
 
 @pytest.fixture(params=[1, 2, 0], ids=["tcgen05-fullrow", "tcgen05", "mmasync"])
 def prefill_impl(request, b200, native_lib):
-    """The tcgen05 product kernel with two softmax threads per query row (default) and with one (option
-    prefill_full_row = 1), and the mma.sync bring-up kernel (test builds only)."""
+    """The tensor-core product kernel (wgmma on sm_90a; the ids keep the variant names the suite has
+    always used) with the request-major work order (option prefill_order = 1) and with the size-sorted
+    order (default), and the mma.sync bring-up kernel (test builds only)."""
     try:
         prev = b200._cabi.set_option("prefill_impl", 0 if request.param == 0 else 1)
     except b200._cabi.B200NativeError:
         pytest.skip("cross-check kernel not in this build (B200_BUILD_BRINGUP=1)")
-    prev_rows = b200._cabi.set_option("prefill_full_row", 1 if request.param == 1 else 0)
+    prev_order = b200._cabi.set_option("prefill_order", 1 if request.param == 1 else 0)
     yield request.param
     b200._cabi.set_option("prefill_impl", prev)
-    b200._cabi.set_option("prefill_full_row", prev_rows)
+    b200._cabi.set_option("prefill_order", prev_order)
 
 
 PREFILL_LENS = {
@@ -320,7 +319,7 @@ def test_decode_full_size_properties(b200, native_lib, decode_impl):
 @pytest.mark.parametrize("phase", ["decode", "prefill"])
 def test_attention_against_flashinfer_golden(b200, native_lib, phase):
     """Product path vs the outputs FlashInfer (fa2 wrappers, the reference's parity oracle) produced
-    for the same inputs on a B200 (tests/golden/make_flashinfer_golden.py)."""
+    for the same inputs (tests/golden/make_flashinfer_golden.py)."""
     from pathlib import Path
 
     from helpers import World
@@ -512,14 +511,14 @@ def test_attention_against_reference_gpu_goldens(b200, native_lib, case):
 # ------------------------------------------------------------------ per-CTA unit lists longer than their smem cache
 def test_decode_more_units_than_the_smem_unit_cache(b200, native_lib):
     """kMaxUnitsSmem = 96 units per CTA are decoded into shared memory; beyond that the roles decode
-    units on the fly (attn_decode_tc.cu unit_at).  2000 short requests x 8 kv heads = 16 000 units > 96 x 148."""
+    units on the fly (attn_decode_tc.cu unit_at).  2000 short requests x 8 kv heads = 16 000 units > 96 x 132."""
     rnd = random.Random(11)
     lens = [(n - 1, n) for n in (rnd.randint(1, 9) for _ in range(2000))]
     _run_case(b200, page_size=16, hq=16, hkv=8, lens=lens, phase="decode", max_seq=32)
 
 
 def test_prefill_more_units_than_the_smem_unit_cache(b200, native_lib):
-    """Same for the prefill kernel (kMaxUnitsSmem = 64): 1250 two-token extends x 8 kv heads = 10 000 units."""
+    """Same for the prefill kernel (kMaxUnitsSmem = 64): 1250 two-token extends x 16 query heads = 20 000 units."""
     lens = [(3, 5)] * 1250
     _run_case(b200, page_size=1, hq=16, hkv=8, lens=lens, phase="prefill", max_seq=32)
 

@@ -254,7 +254,7 @@ def _bf(a):
 
 def test_rope_and_norms_bit_identical_to_flashinfer(b200, native_lib):
     """Golden outputs of the FlashInfer ops the reference binds (layers/rotary.py:45, norm.py:16-38):
-    the B200 kernels reproduce them bit for bit."""
+    the project's kernels reproduce them bit for bit."""
     fi = _fi()
     hq, hkv, d = 4, 2, 128
     x = _bf(fi["rope_x"])

@@ -32,8 +32,8 @@ def test_abi_version_and_helpers(b200, native_lib):
     assert native_lib.b200_decode_plan_ints(256) == 4 + 257 + 16 * 256
     assert native_lib.b200_attn_workspace_bytes(256, 16, 128) > 256 * 16 * 16 * 128 * 4
     assert native_lib.b200_launch_count() == 0  # nothing was launched on this CPU box
-    prev = b200._cabi.set_option("decode_lookahead", 3)
-    assert b200._cabi.set_option("decode_lookahead", prev) == 3
+    prev = b200._cabi.set_option("decode_plan_target", 3)
+    assert b200._cabi.set_option("decode_plan_target", prev) == 3
     # the cross-check kernels (cp.async decode, mma.sync prefill) are not in the product build
     import os
 

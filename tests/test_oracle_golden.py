@@ -141,7 +141,7 @@ def test_norm_oracle_properties():
 
 # ------------------------------------------------------------------ floating-point side
 # tests/golden/flashinfer_golden.npz: inputs + outputs of FlashInfer 0.6.11.post2 called exactly as
-# the reference's call sites do, produced on a B200 by tests/golden/make_flashinfer_golden.py.
+# the reference's call sites do, produced by tests/golden/make_flashinfer_golden.py.
 FI = np.load(Path(__file__).parent / "golden" / "flashinfer_golden.npz")
 
 

@@ -3,7 +3,7 @@
 decode_fused_combine) over decode iterations of cfg1 with different live batch sizes, one process.
 
     python tools/decode_sweep.py --iters 100,500,800,900,980,1015 --targets 1,2,4 --nosplit 0,50,75,100 --fused 0,1,2
-    python tools/decode_sweep.py --graph --layers 28 --opts "decode_defer_epilogue=0;decode_defer_epilogue=1"
+    python tools/decode_sweep.py --graph --layers 28 --opts "decode_fused_combine=0;decode_fused_combine=1"
 """
 import argparse
 import importlib

@@ -4,7 +4,7 @@ Qwen3-0.6B shape): achieved GB/s = algorithmic bytes (rows read + written, weigh
 time, against the measured HBM peak.  Inputs are rotated over buffers larger than L2 so every launch is
 cold.  Run plain for the timing JSON, or under
   ncu --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum --clock-control none
-for the per-launch DRAM traffic (profiles/r02_ncu_elementwise.csv).
+for the per-launch DRAM traffic.
 
     python tools/elementwise_bench.py [--out gpurun_out/elementwise.json] [--reps 20]
 """

@@ -2,7 +2,7 @@
 """Same-box comparison with the reference's two GPU attention paths on the bench workload
 (BASELINE.md section 2): R-fi = FlashInfer fa2 wrappers with page_size 1 (python/minisgl/attention/
 fi.py), R-trtllm = FlashInfer's TRT-LLM-gen sm100a FMHA cubins with page_size 64
-(python/minisgl/attention/trtllm.py; what the reference auto-selects on B200).  FlashInfer is called
+(python/minisgl/attention/trtllm.py; what the reference auto-selects on sm_100).  FlashInfer is called
 with exactly the keyword usage of those files; the reference's own tvm-ffi store kernel cannot be
 built here, so the KV append in front of the FlashInfer calls uses our store kernel (same bytes).
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""In-situ drop-in check: the UNMODIFIED reference (`minisgl`, pip-installed into the git-ignored
-baseline/_ref) drives the attention backend through its own `LLM` -> `Scheduler` -> `Engine` ->
+"""In-situ drop-in check: the UNMODIFIED reference (`minisgl`, copied into the git-ignored
+oracle/_ref/minisgl_site by build(), see oracle/reference_site.py) drives the attention backend through its own `LLM` -> `Scheduler` -> `Engine` ->
 `GraphRunner` -> `CacheManager` stack, once per attention backend, and the bf16 logits of every
 forward (prefill, chunked prefill, radix-hit extend, graph-replayed padded decode) are compared.
 
@@ -8,7 +8,7 @@ forward (prefill, chunked prefill, radix-hit extend, graph-replayed padded decod
       python tools/insitu.py child --attn b200 --page-size 64 --out /tmp/x.pt [--force /tmp/fi.pt]
              [--patch none|flashinfer|model] [--patch-kernels]
   driver mode (spawns the children, compares, prints + writes a JSON summary):
-      python tools/insitu.py run --out gpurun_out/insitu_summary.json
+      python tools/insitu.py run --out insitu_summary.json
 
 What the reference is asked to do (reference file:line of the code that runs):
   * `LLM.generate` twice (llm/llm.py:81-98): round A fills the radix cache, round B re-uses two of
@@ -37,10 +37,8 @@ import time
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
-# the unmodified reference, pip-installed (--no-deps --target) into a git-ignored directory that travels to
-# the GPU box with the snapshot: oracle/_ref/minisgl_site (preferred) or baseline/_ref
-REF = next((d for d in (ROOT / "oracle" / "_ref" / "minisgl_site", ROOT / "baseline" / "_ref")
-            if (d / "minisgl" / "core.py").exists()), ROOT / "oracle" / "_ref" / "minisgl_site")
+# the unmodified reference, copied by build() into a git-ignored directory (oracle/reference_site.py)
+REF = ROOT / "oracle" / "_ref" / "minisgl_site"
 
 QWEN3_0_6B = {  # public HF config of Qwen/Qwen3-0.6B (SURVEY.md section 8)
     "architectures": ["Qwen3ForCausalLM"], "model_type": "qwen3", "hidden_size": 1024,
@@ -80,6 +78,8 @@ def child(args) -> None:
     sys.path.insert(0, str(REF))
     sys.path.insert(0, str(ROOT))
     os.environ.setdefault("FLASHINFER_WORKSPACE_BASE", str(ROOT / "oracle" / "_ref" / "flashinfer_ws"))
+    if args.fi_tensor_cores:  # the reference's own switch (env.py FLASHINFER_USE_TENSOR_CORES, fi.py use_tensor_cores)
+        os.environ["MINISGL_FLASHINFER_USE_TENSOR_CORES"] = "1"
     import torch
 
     model_dir = Path(tempfile.mkdtemp(prefix="q3cfg_"))
@@ -259,7 +259,7 @@ def logits_bit_identical(path_a: str, path_b: str) -> bool:
 
 
 def run_child(tag: str, out_dir: Path, attn: str, page_size: int, force: "str | None", patch: str = "none",
-              patch_kernels: bool = False, layers: int = 28, timeout: int = 600) -> str:
+              patch_kernels: bool = False, layers: int = 28, timeout: int = 600, fi_tensor_cores: bool = False) -> str:
     out = out_dir / f"{tag}.pt"
     cmd = [sys.executable, str(Path(__file__).resolve()), "child", "--attn", attn, "--page-size", str(page_size),
            "--out", str(out), "--patch", patch, "--layers", str(layers)]
@@ -267,6 +267,8 @@ def run_child(tag: str, out_dir: Path, attn: str, page_size: int, force: "str | 
         cmd += ["--force", force]
     if patch_kernels:
         cmd += ["--patch-kernels"]
+    if fi_tensor_cores:
+        cmd += ["--fi-tensor-cores"]
     t0 = time.time()
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=timeout, cwd=str(ROOT))
     log = res.stdout.decode(errors="replace")
@@ -283,13 +285,15 @@ def run(args) -> dict:
     summary = {"model": f"Qwen3-0.6B shape, {L} layers, dummy weights (engine.py:140-144), bf16",
                "criterion": "per row max|a-b| / max|b| over the vocabulary, worst row of all forwards"}
     # canonical free-running run: the reference's FlashInfer path, page_size 1 (fi.py only knows page 1);
-    # every other run is teacher-forced with its tokens
+    # every other run is teacher-forced with its tokens.  The reference's second path for the spread it shows
+    # against itself is its FlashInfer backend with tensor-core decode (16-bit P, as the reference runs it for
+    # GQA >= 4 models, fi.py use_tensor_cores); its TRT-LLM-gen path ships sm_100 kernels only.
     fi1 = run_child("fi_p1", out_dir, "fi", 1, None, layers=L)
     runs, errors = {"fi_p1": fi1}, {}
     plan = [
         ("b200_p1", dict(attn="b200", page_size=1)),
         ("fi_p64", dict(attn="fi", page_size=64)),
-        ("trtllm_p64", dict(attn="trtllm", page_size=64)),
+        ("fi_tc_p64", dict(attn="fi", page_size=64, fi_tensor_cores=True)),
         ("b200_p64", dict(attn="b200", page_size=64)),
         ("b200_p64_patched", dict(attn="b200", page_size=64, patch="model", patch_kernels=True)),
         ("fi_p64_fipatched", dict(attn="fi", page_size=64, patch="flashinfer", patch_kernels=True)),
@@ -303,8 +307,8 @@ def run(args) -> dict:
     pairs = {
         "b200_vs_fi_page1": ("b200_p1", "fi_p1"),
         "b200_vs_fi_page64": ("b200_p64", "fi_p64"),
-        "trtllm_vs_fi_page64": ("trtllm_p64", "fi_p64"),
-        "b200_vs_trtllm_page64": ("b200_p64", "trtllm_p64"),
+        "fi_tc_vs_fi_page64": ("fi_tc_p64", "fi_p64"),
+        "b200_vs_fi_tc_page64": ("b200_p64", "fi_tc_p64"),
         "b200_patched_vs_fi_page64": ("b200_p64_patched", "fi_p64"),
         "b200_patched_vs_b200_page64": ("b200_p64_patched", "b200_p64"),
     }
@@ -337,12 +341,13 @@ def main() -> None:
     c.add_argument("--force", default=None)
     c.add_argument("--patch", default="none", choices=["none", "flashinfer", "model"])
     c.add_argument("--patch-kernels", action="store_true")
+    c.add_argument("--fi-tensor-cores", action="store_true")
     r = sub.add_parser("run")
     r.add_argument("--out", default=None)
     r.add_argument("--layers", type=int, default=28)
     args = ap.parse_args()
     if not reference_available():
-        raise SystemExit("the reference is not installed: python -m pip install --no-index --no-build-isolation --no-deps --target oracle/_ref/minisgl_site <copy of the reference>")
+        raise SystemExit("the reference is not installed: MINISGL_REFERENCE=<reference checkout> python -m oracle.reference_site")
     child(args) if args.mode == "child" else run(args)
 
 

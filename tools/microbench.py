@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Kernel-level micro-benchmark on the bench workload (one decode iteration of cfg1, a few layers):
-used under ncu for the per-kernel captures in profiles/ and stand-alone for quick timing.
+used under ncu for per-kernel captures and stand-alone for quick timing.
 
     python tools/microbench.py decode --iter 500 --layers 4 --reps 5
     python tools/microbench.py prefill --layers 2

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Turn an Nsight Compute report into the small JSON summaries kept under profiles/.
+"""Turn an Nsight Compute report into a small JSON summary.
 
     ncu -i gpurun_out/decode_tc.ncu-rep --page raw --csv > /tmp/raw.csv     # done by this script
-    python tools/ncu_summary.py gpurun_out/decode_tc.ncu-rep profiles/r01_ncu_decode_tc_summary.json
+    python tools/ncu_summary.py decode_tc.ncu-rep decode_tc_summary.json
 """
 import csv
 import io

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Per-kernel SASS opcode census of libb200attn.so (cuobjdump -sass): the evidence that the hot ops run on
-tcgen05 / TMA / TMEM (UTCHMMA, UTMALDG[.GATHER4], UTMASTG[.SCATTER4], LDTM, STTM, UTCBAR) and that the product
-build has no legacy mma.sync (HMMA.16816) path.
+wgmma / TMA (HGMMA, UTMALDG, UTMASTG, USETMAXREG) and that the product build has no legacy mma.sync
+(HMMA.16816) path.
 
-    python tools/sass_opcodes.py > profiles/r02_sass_opcodes.txt
+    python tools/sass_opcodes.py > sass_opcodes.txt
 """
 import collections
 import re
@@ -13,8 +13,8 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
 LIB = ROOT / "mini-sglang_b200" / "libb200attn.so"
-WATCH = ["UTCHMMA", "UTCBAR", "UTMALDG", "UTMASTG", "UTMAPF", "LDTM", "STTM", "HMMA", "LDGSTS", "SYNCS", "MUFU.EX2",
-         "USETMAXREG", "ACQBULK", "CREDUX", "LDG", "STG", "LDS", "STS", "RED", "ATOM", "BAR", "FFMA", "SHFL"]
+WATCH = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAPF", "HMMA", "LDGSTS", "SYNCS", "MUFU.EX2",
+         "USETMAXREG", "ACQBULK", "LDG", "STG", "LDS", "STS", "RED", "ATOM", "BAR", "FFMA", "SHFL"]
 
 
 def main():
@@ -31,7 +31,7 @@ def main():
             per[fn][m.group(1)] += 1
     demangled = subprocess.run(["c++filt"], input="\n".join(per), capture_output=True, text=True).stdout.splitlines()
     total = collections.Counter()
-    print(f"# {LIB.name}: SASS opcode census per kernel (cuobjdump -sass), sm_100a")
+    print(f"# {LIB.name}: SASS opcode census per kernel (cuobjdump -sass), sm_90a")
     for (fn, cnt), name in zip(per.items(), demangled):
         short = re.sub(r"\(.*", "", name)
         n = sum(cnt.values())
@@ -39,13 +39,13 @@ def main():
         for op, c in cnt.items():
             for w in WATCH:
                 if op == w or op.startswith(w + ".") or (w in ("UTMALDG", "UTMASTG") and op.startswith(w)):
-                    key = op if w in ("UTMALDG", "UTMASTG", "UTCHMMA", "LDTM", "STTM", "HMMA") else w
+                    key = op if w in ("UTMALDG", "UTMASTG", "HGMMA", "HMMA") else w
                     groups[key] += c
                     break
         total.update(groups)
         keys = [k for k in groups if not k.startswith(("LDG", "STG", "LDS", "STS", "BAR", "FFMA", "SHFL", "RED", "ATOM", "SYNCS"))]
         print(f"\n{short}\n  instructions: {n}")
-        print("  " + ", ".join(f"{k}: {groups[k]}" for k in sorted(keys)) if keys else "  (no tensor / TMA / TMEM opcodes)")
+        print("  " + ", ".join(f"{k}: {groups[k]}" for k in sorted(keys)) if keys else "  (no tensor / TMA opcodes)")
         print("  " + ", ".join(f"{k}: {groups[k]}" for k in sorted(groups) if k not in keys))
     print("\n# totals over the library")
     print(", ".join(f"{k}: {v}" for k, v in sorted(total.items())))
