@@ -54,6 +54,9 @@ B200_API int b200_device_supported(void);
  *   "decode_early_kv": 1 (default) = a decode launch that is being captured into a CUDA graph lets its TMA
  *       producers stream K/V before the predecessor kernel has finished (programmatic dependent launch; the
  *       metadata and this layer's pool slice are not written inside the graph); 0 = always wait first.
+ *   "decode_exact_tail": 1 (default) = at page sizes >= 8 the decode kernel loads the page piece that holds
+ *       the end of a KV range only up to its last valid row (8-row boxes); 0 = that piece is loaded whole.
+ *       Outputs are bit-identical either way.
  *   "decode_plan_target": when splitting, aim at target * CTA-hint / kv_heads (request, chunk) items (default 2).
  *   "decode_plan_nosplit": no split-KV once bs * kv_heads * 100 >= value * CTA-hint (default 75; 0 = always split).
  * Returns the previous value, or -1 for an unknown name. */

@@ -8,7 +8,9 @@
 //            128-key tile), data lands directly in the 128-byte-swizzled layout wgmma consumes.
 //            * page_size >= 8 ("box mode", warp 0 = K, warp 1 = V): the slots of a page are contiguous
 //              rows of the pool, so one tiled TMA box of min(page_size, 64) rows x 128 B is issued per
-//              page piece -- 4 instructions per tile and half at page_size 64.
+//              page piece -- 4 instructions per tile and half at page_size 64.  The piece holding the
+//              end of the KV range is loaded as 8-row boxes up to its last valid row, and pieces past
+//              the end are not loaded at all, so no more than 7 rows past the end come from HBM.
 //            * page_size < 8 ("row mode", all four warps): one single-row TMA box per token row and
 //              half; rows past the end of the KV range are out-of-range rows (zero filled), so stale
 //              pool memory is never multiplied in.
@@ -95,6 +97,7 @@ struct Params {
   int bs, hq, hkv;
   int num_slots;
   int box_rows;  // rows per tiled TMA box (8..64, divides page_size); 0 = row mode
+  int exact_tail;  // box mode: the box holding the end of a range loads only its valid rows (8-row granules)
   int fused_combine;  // 1: last-arriving unit merges the split-KV partials in this launch
   float scale_log2;
   T* out;
@@ -143,7 +146,9 @@ __global__ void __launch_bounds__(kThreads, 1)
 attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map_k,
                       const __grid_constant__ CUtensorMap map_v,
                       const __grid_constant__ CUtensorMap box_k,
-                      const __grid_constant__ CUtensorMap box_v) {
+                      const __grid_constant__ CUtensorMap box_v,
+                      const __grid_constant__ CUtensorMap tail_k,
+                      const __grid_constant__ CUtensorMap tail_v) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B-swizzled tiles
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -181,6 +186,8 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     prefetch_tensormap(&map_v);
     prefetch_tensormap(&box_k);
     prefetch_tensormap(&box_v);
+    prefetch_tensormap(&tail_k);
+    prefetch_tensormap(&tail_v);
   }
   // PDL: everything above may overlap the tail of the previous kernel in the stream.
   //  * p.early == 0 (eager launches): wait here -- from here on the results of every kernel before this one
@@ -277,27 +284,41 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             tma_load_2d(dst + 384, gmap, fb, col, cur.w);
           }
         } else {
-          // ---- box mode: instruction idx = (box, half); a box is rb consecutive positions of one page
+          // ---- box mode: lane = (box, half); a box is rb consecutive positions of one page
           const int n_instr = (kTileN / rb) * 2;  // <= 32
+          const CUtensorMap* tmap = kind == 0 ? &tail_k : &tail_v;
           for (int t = 0; t < u.n_tiles; ++t, ++tile_count) {
             const uint32_t stage = tile_count % kStages, phase = (tile_count / kStages) & 1;
             const int tile_begin = u.kv_begin + t * kTileN;
             const int box = lane >> 1, half = lane & 1;
             const int pb = tile_begin + box * rb;
+            // Rows this lane loads.  Exact tail: a box wholly inside the range is one rb-row box, the box
+            // holding the end of the range is cut to its valid rows rounded up to 8-row boxes, and a box
+            // wholly past the end is not issued.  Otherwise every box is loaded whole: one reaching past
+            // the end reads the rest of its page from HBM, one wholly past the end gets out-of-range rows.
+            // Rows of the stage that are not loaded keep older contents: the consumer warps mask those K
+            // rows by position and zero those V rows before PV.
+            const int left = u.kv_end_tc - pb;
+            int rows = 0;
+            if (lane < n_instr) rows = !p.exact_tail ? rb : (left <= 0 ? 0 : min(rb, (left + 7) & ~7));
             // slot of the box's first row, loaded before the wait so its latency overlaps
             int first_slot = p.num_slots;
-            if (lane < n_instr && pb < u.kv_end_tc) first_slot = __ldg(slots + pb);
+            if (lane < n_instr && left > 0) first_slot = __ldg(slots + pb);
+            // the stage's transaction bytes are exactly the rows the lanes issue below
+            const uint32_t tx_bytes = __reduce_add_sync(0xffffffffu, (uint32_t)rows) * 128u;
             mbar_wait(bar(empty0 + stage), phase ^ 1);
-            if (lane == 0) mbar_arrive_expect_tx(bar(full0 + stage), kStageBytes);
+            if (lane == 0) mbar_arrive_expect_tx(bar(full0 + stage), tx_bytes);
             __syncwarp();
-            if (lane < n_instr) {
+            if (rows > 0) {
               const uint32_t dst = ring + stage * kStageBytes + half * kHalfBytes + box * rb * 128;
               const uint32_t fb = bar(full0 + stage);
               const int col = col0 + half * 64;
-              // A box reaching past the end of the range still lies inside the request's page; the
-              // extra K rows are masked by position and the extra V rows are zeroed in smem by the
-              // consumer warps before PV.  A box wholly past the end gets an out-of-range row => zeros.
-              tma_load_2d(dst, bmap, fb, col, first_slot);
+              if (rows == rb) {
+                tma_load_2d(dst, bmap, fb, col, first_slot);
+              } else {
+                // the rows of a box are consecutive slots of one page
+                for (int r = 0; r < rows; r += 8) tma_load_2d(dst + r * 128, tmap, fb, col, first_slot + r);
+              }
             }
           }
         }
@@ -443,8 +464,9 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           }
           const int n_valid = u.kv_end_tc - (u.kv_begin + j * kTileN);  // >= 1
           if (p.box_rows > 0 && n_valid < kTileN) {
-            // box mode, last tile of the range: the V rows past the end hold whatever the page holds
-            // (possibly NaN bit patterns): zero them so that 0 * garbage cannot reach the output
+            // box mode, last tile of the range: the V rows past the end hold the rest of the page or
+            // an earlier tile of this stage (possibly NaN bit patterns): zero them so that 0 * garbage
+            // cannot reach the output
             mbar_wait(bar(kFullV + stage), sphase);
             uint8_t* vt = smem + Smem::vring + stage * kStageBytes;
             for (int idx = ct; idx < (kTileN - n_valid) * 16; idx += 128) {
@@ -718,7 +740,8 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
 
 template <typename T, int G>
 static int launch_g(const Params<T>& p, const CUtensorMap& mk, const CUtensorMap& mv,
-                    const CUtensorMap& bk, const CUtensorMap& bv, cudaStream_t st) {
+                    const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& tk,
+                    const CUtensorMap& tv, cudaStream_t st) {
   const size_t smem = Smem::total + 1024;
   static bool configured = false;
   if (!configured) {
@@ -726,7 +749,7 @@ static int launch_g(const Params<T>& p, const CUtensorMap& mk, const CUtensorMap
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(attn_decode_tc_kernel<T, G>, dim3(num_sms()), dim3(kThreads), smem, st, p, mk, mv, bk, bv));
+  B200_CHECK_CUDA(launch_pdl(attn_decode_tc_kernel<T, G>, dim3(num_sms()), dim3(kThreads), smem, st, p, mk, mv, bk, bv, tk, tv));
   B200_POST_LAUNCH();
   if (!p.fused_combine) {
     B200_CHECK_CUDA(launch_pdl(attn_combine_kernel<T>, dim3(p.bs, p.hq), dim3(kHeadDim), 0, st,
@@ -748,15 +771,21 @@ static int launch(const Params<T>& p, cudaStream_t st) {
     if (int rc = get_tensor_map_2d(&bk, p.k_cache, p.num_slots, cols, cols * 2, 64, p.box_rows, bf16)) return rc;
     if (int rc = get_tensor_map_2d(&bv, p.v_cache, p.num_slots, cols, cols * 2, 64, p.box_rows, bf16)) return rc;
   }
+  // 8-row boxes for the last page piece of a range (exact tail)
+  CUtensorMap tk = bk, tv = bv;
+  if (p.box_rows > 8) {
+    if (int rc = get_tensor_map_2d(&tk, p.k_cache, p.num_slots, cols, cols * 2, 64, 8, bf16)) return rc;
+    if (int rc = get_tensor_map_2d(&tv, p.v_cache, p.num_slots, cols, cols * 2, 64, 8, bf16)) return rc;
+  }
   switch (p.hq / p.hkv) {
-    case 1: return launch_g<T, 1>(p, mk, mv, bk, bv, st);
-    case 2: return launch_g<T, 2>(p, mk, mv, bk, bv, st);
-    case 3: return launch_g<T, 3>(p, mk, mv, bk, bv, st);
-    case 4: return launch_g<T, 4>(p, mk, mv, bk, bv, st);
-    case 5: return launch_g<T, 5>(p, mk, mv, bk, bv, st);
-    case 6: return launch_g<T, 6>(p, mk, mv, bk, bv, st);
-    case 7: return launch_g<T, 7>(p, mk, mv, bk, bv, st);
-    case 8: return launch_g<T, 8>(p, mk, mv, bk, bv, st);
+    case 1: return launch_g<T, 1>(p, mk, mv, bk, bv, tk, tv, st);
+    case 2: return launch_g<T, 2>(p, mk, mv, bk, bv, tk, tv, st);
+    case 3: return launch_g<T, 3>(p, mk, mv, bk, bv, tk, tv, st);
+    case 4: return launch_g<T, 4>(p, mk, mv, bk, bv, tk, tv, st);
+    case 5: return launch_g<T, 5>(p, mk, mv, bk, bv, tk, tv, st);
+    case 6: return launch_g<T, 6>(p, mk, mv, bk, bv, tk, tv, st);
+    case 7: return launch_g<T, 7>(p, mk, mv, bk, bv, tk, tv, st);
+    case 8: return launch_g<T, 8>(p, mk, mv, bk, bv, tk, tv, st);
     default:
       set_error("attn_decode: GQA group size %d not supported (1..8)", p.hq / p.hkv);
       return 1;
@@ -767,6 +796,7 @@ static int launch(const Params<T>& p, cudaStream_t st) {
 
 extern std::atomic<int> g_decode_fused_combine;
 extern std::atomic<int> g_decode_early_kv;
+extern std::atomic<int> g_decode_exact_tail;
 bool decode_plan_is_unsplit(int bs, int num_kv_heads, int ctas);  // metadata.cu
 
 // entry used by b200_attn_decode (attn_decode.cu)
@@ -801,7 +831,8 @@ int launch_decode_tc(const void* q, int64_t q_rs, const void* k, int64_t k_rs, c
 #define RUN(T_)                                                                                   \
   dtc::Params<T_> p{(const T_*)q, q_rs, (const T_*)k, k_rs, (const T_*)v, v_rs, (T_*)k_cache,     \
                     (T_*)v_cache, out_loc, slot_table, st_stride, seq_lens, plan, bs, hq, hkv,    \
-                    (int)num_slots, box_rows, fused, scale_log2, (T_*)out,                        \
+                    (int)num_slots, box_rows, g_decode_exact_tail.load() ? 1 : 0, fused, scale_log2, \
+                    (T_*)out,                                                                     \
                     part_o, part_ml, counters, early, fuse, (const T_*)qw, (const T_*)kw, eps, positions, cos_sin};  \
   return dtc::launch<T_>(p, st)
   if (dtype == B200_DTYPE_BF16) {

@@ -35,6 +35,7 @@ std::atomic<int> g_decode_plan_nosplit{75};  // no split once bs * kv_heads * 10
 // combine launch at all), 2 = in-kernel exactly when the policy above does not split.
 std::atomic<int> g_decode_fused_combine{1};
 std::atomic<int> g_decode_early_kv{1};  // captured decode launches stream K/V without waiting for the predecessor
+std::atomic<int> g_decode_exact_tail{1};  // box mode: the last page piece of a range loads only its valid rows
 }
 
 extern "C" int b200_abi_version(void) { return 7; }
@@ -60,6 +61,7 @@ extern "C" int b200_set_option(const char* name, int value) {
   if (name != nullptr && std::strcmp(name, "decode_plan_nosplit") == 0) return b200::g_decode_plan_nosplit.exchange(value);
   if (name != nullptr && std::strcmp(name, "decode_early_kv") == 0) return b200::g_decode_early_kv.exchange(value);
   if (name != nullptr && std::strcmp(name, "decode_fused_combine") == 0) return b200::g_decode_fused_combine.exchange(value);
+  if (name != nullptr && std::strcmp(name, "decode_exact_tail") == 0) return b200::g_decode_exact_tail.exchange(value);
   return -1;
 }
 
