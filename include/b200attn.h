@@ -94,14 +94,16 @@ B200_API int b200_index_rows(const void* weights, int64_t weight_row_stride_byte
  *     and the per-head q/k norm at M/layers/attention.py:50-53.
  *     x viewed as [rows, heads, dim]: element (r,h,i) at x + r*x_row_stride + h*x_head_stride + i
  *     (strides in elements); plain 2-D input uses heads = 1.  out may alias x (in place).
- *     y = float(x) * rsqrt(mean(x^2) + eps) * float(w), one rounding.  dim % 8 == 0, dim <= 8192.
+ *     y = float(x) * rsqrt(mean(x^2) + eps) * float(w), one rounding.  dim % 8 == 0; dim <= 16384
+ *     (heads == 1), dim in {64, 128, 256} for heads > 1.  A wider dim is rejected before any launch.
  * ------------------------------------------------------------------------------------- */
 B200_API int b200_rmsnorm(void* out, const void* x, const void* weight, int64_t rows, int heads, int dim,
                  int64_t x_row_stride, int64_t x_head_stride, int64_t out_row_stride,
                  int64_t out_head_stride, float eps, int dtype, void* stream);
 
 /* flashinfer.fused_add_rmsnorm(x, residual, w, eps) at M/layers/norm.py:32-38 (both in place):
- * s = x + residual (fp32); residual <- round(s); x <- round(s * rsqrt(mean(s^2)+eps) * w). */
+ * s = x + residual (fp32); residual <- round(s); x <- round(s * rsqrt(mean(s^2)+eps) * w).
+ * dim % 8 == 0, dim <= 16384. */
 B200_API int b200_fused_add_rmsnorm(void* x, void* residual, const void* weight, int64_t rows, int dim,
                            int64_t x_row_stride, int64_t res_row_stride, float eps, int dtype,
                            void* stream);
@@ -232,7 +234,8 @@ B200_API int b200_attn_prefill(const void* q, int64_t q_row_stride, const void* 
  *     and b200_ar_create receives the `world` base pointers in rank order (bases[rank] = own region;
  *     opened_mask[i] != 0 marks pointers b200_ar_destroy must unmap).
  *
- *     b200_ar_allreduce: x [rows, dim] (row stride in elements), 16-bit floats, rows*dim*2 <= max_bytes.
+ *     b200_ar_allreduce: x [rows, dim] (row stride in elements), 16-bit floats, dim % 8 == 0, dim <= 8192,
+ *       rows*dim*2 <= max_bytes.
  *       residual == weight == NULL:  out <- sum over ranks of x (fp32 accumulation in rank order, one
  *         rounding; identical bits on every rank); out may alias x.
  *       else:  y = that sum; residual <- round(y + residual); out <- round((y + residual) *

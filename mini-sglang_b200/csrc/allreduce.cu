@@ -316,7 +316,7 @@ extern "C" int b200_ar_alloc(size_t bytes, void** ptr) {
   B200_CHECK_CUDA(cudaMalloc(ptr, bytes));
   // data region: every 16-bit lane = the sentinel (negative zero); trailing 256 bytes (epoch, done counter) = 0
   ar::fill_u32_kernel<<<256, 256>>>(static_cast<uint32_t*>(*ptr), (bytes - 256) / 4, ar::kSentinel2);
-  B200_CHECK_CUDA(cudaPeekAtLastError());
+  B200_CHECK_CUDA(cudaGetLastError());
   B200_CHECK_CUDA(cudaMemset(static_cast<char*>(*ptr) + bytes - 256, 0, 256));
   B200_CHECK_CUDA(cudaDeviceSynchronize());
   return 0;

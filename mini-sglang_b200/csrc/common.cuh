@@ -25,21 +25,24 @@ extern std::atomic<uint64_t> g_launch_count;
     }                                \
   } while (0)
 
+// A failed runtime call also records its error as the thread's last error; it is cleared here, so that it
+// is reported by this call only and not again by the next launch check (sticky errors stay sticky).
 #define B200_CHECK_CUDA(expr)                                                       \
   do {                                                                              \
     cudaError_t err__ = (expr);                                                     \
     if (err__ != cudaSuccess) {                                                     \
+      (void)cudaGetLastError();                                                     \
       ::b200::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(err__),  \
                         __FILE__, __LINE__);                                        \
       return 2;                                                                     \
     }                                                                               \
   } while (0)
 
-// call after every <<< >>> launch
+// call after every <<< >>> launch: reports (and clears) a launch error once
 #define B200_POST_LAUNCH()                        \
   do {                                            \
     ::b200::g_launch_count.fetch_add(1);          \
-    B200_CHECK_CUDA(cudaPeekAtLastError());       \
+    B200_CHECK_CUDA(cudaGetLastError());          \
   } while (0)
 
 inline int num_sms() {

@@ -186,12 +186,11 @@ static int launch_rmsnorm(void* out, const void* x, const void* w, int64_t rows,
     return 0;
   }
   B200_CHECK_ARG(heads == 1, "rmsnorm: multi-head rows need dim in {64,128,256}, got %d", dim);
+  // one 16-byte chunk per thread up to 512 chunks, two beyond: at most 1024 threads, i.e. dim <= 16384
   const int chunks = dim / 8;
-  int threads = (int)ceil_div(chunks, 32) * 32;
-  if (threads > 1024) threads = 1024;
-  if (chunks > 512) threads = (int)ceil_div(ceil_div(chunks, 2), 32) * 32;
+  const int threads = (int)ceil_div(chunks > 512 ? ceil_div(chunks, 2) : chunks, 32) * 32;
   const int iters = ceil_div(chunks, threads);
-  B200_CHECK_ARG(iters <= 2, "rmsnorm: dim %d too large (max 16384)", dim);
+  B200_CHECK_ARG(threads <= 1024, "rmsnorm: dim %d too large (max 16384)", dim);
   dim3 grid((unsigned)rows), block(threads);
   if (iters == 1)
     rmsnorm_row_kernel<T, 1, false><<<grid, block, 0, st>>>((T*)out, (const T*)x, nullptr,
@@ -207,12 +206,10 @@ template <typename T>
 static int launch_fused_add_rmsnorm(void* x, void* res, const void* w, int64_t rows, int dim,
                                     int64_t xrs, int64_t rrs, float eps, cudaStream_t st) {
   if (rows == 0) return 0;
-  const int chunks = dim / 8;
-  int threads = (int)ceil_div(chunks, 32) * 32;
-  if (threads > 1024) threads = 1024;
-  if (chunks > 512) threads = (int)ceil_div(ceil_div(chunks, 2), 32) * 32;
+  const int chunks = dim / 8;  // thread <-> chunk mapping of launch_rmsnorm
+  const int threads = (int)ceil_div(chunks > 512 ? ceil_div(chunks, 2) : chunks, 32) * 32;
   const int iters = ceil_div(chunks, threads);
-  B200_CHECK_ARG(iters <= 2, "fused_add_rmsnorm: dim %d too large (max 16384)", dim);
+  B200_CHECK_ARG(threads <= 1024, "fused_add_rmsnorm: dim %d too large (max 16384)", dim);
   dim3 grid((unsigned)rows), block(threads);
   if (iters == 1)
     rmsnorm_row_kernel<T, 1, true><<<grid, block, 0, st>>>((T*)x, (const T*)x, (T*)res,

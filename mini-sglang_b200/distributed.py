@@ -64,8 +64,9 @@ class B200AllReduce:
         torch.distributed.barrier(group=group)  # every rank has mapped every region before the first push
 
     def fits(self, x: torch.Tensor) -> bool:
+        """True when the kernel accepts a contiguous ``x``: anything else goes to the fallback."""
         return x.is_cuda and x.dtype in _DTYPE_CODE and x.dim() >= 1 and x.shape[-1] % 8 == 0 and \
-            x.numel() * x.element_size() <= self.max_bytes
+            x.data_ptr() % 16 == 0 and x.numel() * x.element_size() <= self.max_bytes
 
     def all_reduce(self, x: torch.Tensor, out: Optional[torch.Tensor] = None,
                    residual: Optional[torch.Tensor] = None, weight: Optional[torch.Tensor] = None,

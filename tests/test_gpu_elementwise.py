@@ -123,7 +123,10 @@ def test_indexing_rejects_bad_args(b200, native_lib):
         b200.ops.indexing(torch.zeros(16, 4, device="cuda", dtype=torch.bfloat16), torch.zeros(2, dtype=torch.int32, device="cuda"))
 
 
-@pytest.mark.parametrize("rows,dim", [(1, 1024), (37, 1024), (256, 5120), (19, 8192), (5, 4096), (3, 2048 + 64)])
+# 2-D dims 64 / 128 / 256 take the lane-group kernel (heads = 1); 4104 is the first width with two 16-byte
+# chunks per thread, 16384 the widest row (1024 threads)
+@pytest.mark.parametrize("rows,dim", [(1, 1024), (37, 1024), (256, 5120), (19, 8192), (5, 4096), (3, 2048 + 64),
+                                      (33, 64), (130, 128), (7, 256), (9, 4104), (3, 16384)])
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 def test_rmsnorm_rows(b200, native_lib, rows, dim, dtype):
     torch.manual_seed(rows * dim)
@@ -152,17 +155,56 @@ def test_rmsnorm_per_head_strided(b200, native_lib, heads, d):
     assert torch.equal(bg[:, heads * d :].cpu(), buf[:, heads * d :])  # neighbours untouched
 
 
-@pytest.mark.parametrize("rows,dim", [(1, 1024), (64, 1024), (33, 5120), (7, 8192)])
-def test_fused_add_rmsnorm(b200, native_lib, rows, dim):
+@pytest.mark.parametrize("rows,dim,dtype,strided", [
+    pytest.param(1, 1024, torch.bfloat16, False, id="1-1024"),
+    pytest.param(64, 1024, torch.bfloat16, False, id="64-1024"),
+    pytest.param(33, 5120, torch.bfloat16, False, id="33-5120"),
+    pytest.param(7, 8192, torch.bfloat16, False, id="7-8192"),
+    pytest.param(64, 1024, torch.float16, False, id="fp16-64-1024"),
+    pytest.param(7, 8192, torch.float16, True, id="fp16-7-8192-strided"),
+    pytest.param(5, 1032, torch.bfloat16, True, id="5-1032-strided"),
+    pytest.param(130, 1032, torch.float16, False, id="fp16-130-1032"),
+    pytest.param(9, 4104, torch.bfloat16, False, id="9-4104"),
+    pytest.param(9, 4104, torch.float16, True, id="fp16-9-4104-strided"),
+    pytest.param(3, 16384, torch.bfloat16, True, id="3-16384-strided"),
+    pytest.param(3, 16384, torch.float16, False, id="fp16-3-16384"),
+])
+def test_fused_add_rmsnorm(b200, native_lib, rows, dim, dtype, strided):
     torch.manual_seed(3)
-    x = torch.randn(rows, dim).to(torch.bfloat16)
-    res = (torch.randn(rows, dim) * 2).to(torch.bfloat16)
-    w = (torch.rand(dim) + 0.5).to(torch.bfloat16)
+    x = torch.randn(rows, dim).to(dtype)
+    res = (torch.randn(rows, dim) * 2).to(dtype)
+    w = (torch.rand(dim) + 0.5).to(dtype)
     ref_x, ref_res = o_norm.ref_fused_add_rmsnorm(x, res, w, 1e-6)
-    xg, rg = x.cuda(), res.cuda()
+    if strided:  # rows of wider buffers (row strides dim + 8 and dim + 24); the padding must survive
+        xb, rb = torch.randn(rows, dim + 8).to(dtype).cuda(), torch.randn(rows, dim + 24).to(dtype).cuda()
+        pads = xb[:, dim:].clone(), rb[:, dim:].clone()
+        xg, rg = xb[:, :dim], rb[:, :dim]
+        xg.copy_(x)
+        rg.copy_(res)
+    else:
+        xg, rg = x.cuda(), res.cuda()
     b200.ops.fused_add_rmsnorm(xg, rg, w.cuda(), 1e-6)
     assert torch.equal(rg.cpu().view(torch.int16), ref_res.view(torch.int16))  # residual: exact
     _ulp_close(xg, ref_x)
+    if strided:
+        assert torch.equal(xb[:, dim:], pads[0]) and torch.equal(rb[:, dim:], pads[1])
+
+
+def test_rmsnorm_rejects_rows_wider_than_16384(b200, native_lib):
+    """dim 16392 would need a 1056-thread block: both norms reject it up front, naming the dim, and nothing
+    is left behind that makes the next, valid call fail."""
+    dim = 16392
+    x = torch.randn(2, dim, device="cuda").to(torch.bfloat16)
+    w = torch.ones(dim, device="cuda", dtype=torch.bfloat16)
+    launches = b200._cabi.launch_count()
+    with pytest.raises(RuntimeError, match=str(dim)):
+        b200.ops.rmsnorm(x, w, 1e-6)
+    with pytest.raises(RuntimeError, match=str(dim)):
+        b200.ops.fused_add_rmsnorm(x, x.clone(), w, 1e-6)
+    assert b200._cabi.launch_count() == launches
+    y = (torch.randn(3, 1024) * 3).to(torch.bfloat16)
+    wy = (torch.randn(1024) * 0.5 + 1).to(torch.bfloat16)
+    _ulp_close(b200.ops.rmsnorm(y.cuda(), wy.cuda(), 1e-6), o_norm.ref_rmsnorm(y, wy, 1e-6))
 
 
 @pytest.mark.parametrize("pos_dtype", [torch.int32, torch.int64])

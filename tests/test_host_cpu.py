@@ -67,6 +67,11 @@ def test_build_digest_is_embedded(b200, native_lib):
 def test_allreduce_host_api_validates(b200, native_lib):
     """Set-up half of the all-reduce ABI needs no GPU: region sizing and communicator creation."""
     assert native_lib.b200_ar_region_bytes(8, 1 << 20) >= 2 * 8 * (1 << 20) + 8 * 128 * 4
+    # the layout tests/test_gpu_allreduce_local.py addresses directly: data [2 parities][world][slot], a
+    # reserved area of world * 512 u32 (256-aligned), then 256 bytes holding the epoch and the count-in counter
+    a256 = lambda n: (n + 255) // 256 * 256
+    for w, m in [(1, 1), (1, 4 << 20), (2, 1000), (3, 256), (3, 257), (5, 12345), (8, 1 << 20), (8, (4 << 20) + 8)]:
+        assert native_lib.b200_ar_region_bytes(w, m) == 2 * w * a256(m) + a256(w * 512 * 4) + 256, (w, m)
     bases = (ctypes.c_void_p * 2)(0x1000, 0x2000)
     opened = (ctypes.c_int * 2)(0, 0)
     comm = ctypes.c_void_p()
