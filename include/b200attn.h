@@ -59,7 +59,9 @@ B200_API int b200_device_supported(void);
  *       Outputs are bit-identical either way.
  *   "decode_plan_target": when splitting, aim at target * CTA-hint / kv_heads (request, chunk) items (default 2).
  *   "decode_plan_nosplit": no split-KV once bs * kv_heads * 100 >= value * CTA-hint (default 75; 0 = always split).
- * Returns the previous value, or -1 for an unknown name. */
+ * The bring-up kernels (decode_impl / prefill_impl = 0) exist only in B200_BUILD_BRINGUP=1 builds.
+ * Returns the previous value; -1 for an unknown name or NULL, and for selecting a bring-up kernel the build
+ * does not contain. */
 B200_API int b200_set_option(const char* name, int value);
 
 /* ---------------------------------------------------------------------------------------
@@ -207,7 +209,9 @@ B200_API int b200_attn_decode_fused(const void* q, int64_t q_row_stride, const v
  * q_len = cu_seqlens_q[r+1]-cu_seqlens_q[r] new tokens at kv positions
  * [seq_lens[r]-q_len, seq_lens[r]).  max_seqlen_q is a host-side upper bound (grid sizing).
  * prefill_plan: b200_build_prefill_plan output (work list of the wgmma kernel); NULL selects
- * the mma.sync bring-up kernel (as does b200_set_option("prefill_impl", 0)). */
+ * the mma.sync bring-up kernel (as does b200_set_option("prefill_impl", 0), and so does a GQA group
+ * above 16), which is an error in a build without it.
+ * Every attention entry point checks all its arguments before it launches anything. */
 B200_API int b200_attn_prefill(const void* q, int64_t q_row_stride, const void* k, int64_t k_row_stride,
                       const void* v, int64_t v_row_stride, void* k_cache, void* v_cache,
                       int64_t num_slots, int page_size, const int32_t* out_loc, const int32_t* slot_table,

@@ -23,10 +23,10 @@ SOURCES = [
     "elementwise.cu",
     "index_rows.cu",
     "metadata.cu",
-    "attn_decode.cu",
+    "attn_decode_bringup.cu",
     "attn_decode_tc.cu",
     "tma_host.cu",
-    "attn_prefill.cu",
+    "attn_prefill_bringup.cu",
     "attn_prefill_tc.cu",
     "allreduce.cu",
 ]

@@ -1,0 +1,114 @@
+// The attention contract: what metadata.cu, the decode / prefill kernels and their entry points must agree on
+// (head dim, plan formats, decode workspace layout, TMA boxes over the KV pool) and the arguments an entry
+// point hands to a launcher.
+#pragma once
+#include <cuda.h>
+
+#include "b200attn.h"
+#include "common.cuh"
+
+namespace b200 {
+
+constexpr int kHeadDim = 128;
+
+// ------------------------------------------------------------------------------- decode plan
+// decode_plan = {chunk_tokens, total_chunks, bs, 0, chunk_start[bs + 1], order[total_chunks]}
+constexpr int kPlanHeader = 4;
+constexpr int kMaxSplits = 16;  // chunks per request: metadata.cu never exceeds it, the workspace is sized by it
+
+// order[] entry: r | chunk << 16 | n_chunks << 20   (r < 65536, chunk < 16, n_chunks <= 16)
+struct PlanEntry {
+  int r, c, n_chunks;
+};
+__host__ __device__ __forceinline__ int32_t pack_plan_entry(int r, int c, int n_chunks) {
+  return r | (c << 16) | (n_chunks << 20);
+}
+__host__ __device__ __forceinline__ PlanEntry unpack_plan_entry(int32_t e) {
+  return {e & 0xffff, (e >> 16) & 0xf, (e >> 20) & 0x1f};
+}
+
+// prefill_plan = {n_items, 0, 0, 0, item[n_items]},  item = r | q_tile << 16
+__host__ __device__ __forceinline__ int32_t pack_prefill_item(int r, int q_tile) { return r | (q_tile << 16); }
+__host__ __device__ __forceinline__ int prefill_item_request(int32_t e) { return e & 0xffff; }
+__host__ __device__ __forceinline__ int prefill_item_q_tile(int32_t e) { return (e >> 16) & 0xffff; }
+
+bool decode_plan_is_unsplit(int bs, int num_kv_heads, int ctas);  // metadata.cu: the plan policy's split decision
+
+// -------------------------------------------------------------------------- decode workspace
+// partial o [bs][kMaxSplits][hq][128] | partial (m, l) [bs][kMaxSplits][hq][2] (fp32), the two rounded up to
+// 256 B together, then the split-KV arrival counters [bs][hq] (zero between launches) at the END of the
+// workspace: their place does not depend on bs and they can never overlap the last partials.
+inline size_t decode_workspace_bytes(int max_bs, int hq, int head_dim) {
+  const size_t items = (size_t)max_bs * kMaxSplits * hq;
+  const size_t partials = items * head_dim * sizeof(float) + items * 2 * sizeof(float);
+  const size_t counters = (size_t)max_bs * hq * sizeof(int);
+  return (partials + 255) / 256 * 256 + (counters + 255) / 256 * 256 + 256;
+}
+
+struct DecodeWorkspace {
+  float* part_o;
+  float* part_ml;
+  int* counters;
+};
+inline DecodeWorkspace carve_decode_workspace(void* workspace, size_t workspace_bytes, int bs, int hq) {
+  const size_t items = (size_t)bs * kMaxSplits * hq;
+  float* part_o = reinterpret_cast<float*>(workspace);
+  const size_t cnt_bytes = ((size_t)bs * hq * sizeof(int) + 255) / 256 * 256;
+  char* end = static_cast<char*>(workspace) + workspace_bytes / 256 * 256;
+  return {part_o, part_o + items * kHeadDim, reinterpret_cast<int*>(end - cnt_bytes)};
+}
+
+// ------------------------------------------------------------------------ TMA over the KV pool
+// Rows per tiled TMA box: the largest power of two <= min(page_size, 64) that divides page_size, if that is at
+// least 8 (the slots of a page are consecutive pool rows); 0 = row mode, one single-row box per token.
+inline int box_rows_for(int page_size) {
+  if (page_size < 8) return 0;
+  int rows = 64;
+  while (rows > 8 && page_size % rows != 0) rows >>= 1;
+  return page_size % rows == 0 ? rows : 0;
+}
+
+// Cached tensor map of a 2-D 16-bit [rows, cols] tensor with {box_cols, box_rows} boxes (tma_host.cu).
+int get_tensor_map_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
+                      uint64_t row_stride_bytes, uint32_t box_cols, uint32_t box_rows, bool is_bf16);
+
+// Maps of one layer's K and V pool, [num_slots, hkv * 128] contiguous rows, in boxes of 64 columns x box_rows.
+inline int kv_pool_maps(CUtensorMap* mk, CUtensorMap* mv, const void* k_cache, const void* v_cache,
+                        int64_t num_slots, int hkv, uint32_t box_rows, bool bf16) {
+  const uint64_t cols = (uint64_t)hkv * kHeadDim;
+  if (int rc = get_tensor_map_2d(mk, k_cache, num_slots, cols, cols * 2, 64, box_rows, bf16)) return rc;
+  return get_tensor_map_2d(mv, v_cache, num_slots, cols, cols * 2, 64, box_rows, bf16);
+}
+
+// ------------------------------------------------------------------------- launcher arguments
+// The arguments of b200_attn_decode / b200_attn_decode_fused / b200_attn_prefill in their C ABI order
+// (include/b200attn.h), as the phase's entry point has checked them.
+struct DecodeArgs {
+  const void *q; int64_t q_rs; const void* k; int64_t k_rs; const void* v; int64_t v_rs;
+  void *k_cache, *v_cache; int64_t num_slots; int page_size;
+  const int32_t *out_loc, *slot_table; int64_t st_stride; const int32_t *seq_lens, *plan;
+  int bs, hq, hkv, head_dim; float scale; void* out; void* workspace; size_t workspace_bytes; int dtype;
+  cudaStream_t stream;
+  // b200_attn_decode_fused: q / k are the raw projection rows, normed (weights may be NULL) and roped in the kernel
+  int fuse = 0; const void *qw = nullptr, *kw = nullptr; float eps = 0.f;
+  const int32_t* positions = nullptr; const float* cos_sin = nullptr;
+};
+
+struct PrefillArgs {  // without the workspace, which prefill does not use
+  const void *q; int64_t q_rs; const void* k; int64_t k_rs; const void* v; int64_t v_rs;
+  void *k_cache, *v_cache; int64_t num_slots; int page_size;
+  const int32_t *out_loc, *slot_table; int64_t st_stride; const int32_t *seq_lens, *cu_q, *plan;
+  int bs; int64_t nnz; int max_q; int hq, hkv, head_dim; float scale; void* out; int dtype;
+  cudaStream_t stream;
+};
+
+// Cross-check kernels of B200_BUILD_BRINGUP=1 builds (attn_decode_bringup.cu, attn_prefill_bringup.cu).
+int launch_decode_bringup(const DecodeArgs& a);
+int launch_prefill_bringup(const PrefillArgs& a);
+
+// Swizzled byte offset of 16-byte chunk c (0..15) of row `row` in a bring-up kernel's [rows][256 B] tile.
+__device__ __forceinline__ uint32_t swz(int row, int c) {
+  return (uint32_t)(row * (kHeadDim * 2) + (((c & 8) | ((c ^ row) & 7)) << 4));
+}
+
+}  // namespace b200

@@ -2,7 +2,7 @@
 //
 // Replaces store_kv + BatchDecodeWithPagedKVCacheWrapper.run (python/minisgl/attention/fi.py:185-188)
 // with one persistent launch (+ the split-KV combine).  HBM-bound; algorithmic bytes as in
-// attn_decode.cu.  One CTA per SM, 320 threads, warp-specialised:
+// attn_decode_bringup.cu.  One CTA per SM, 320 threads, warp-specialised:
 //
 //   warps 0-3 TMA producers, 3-stage rings of 32 KB K and 32 KB V tiles (two 64-column halves of a
 //            128-key tile), data lands directly in the 128-byte-swizzled layout wgmma consumes.
@@ -32,24 +32,19 @@
 // The token appended by this launch is handled without touching the pool copy that is being
 // written: its score / value come straight from the k/v inputs on CUDA cores in the epilogue of
 // the unit that owns position kv_len-1 (which also performs the append).
-#include "b200attn.h"
+#include "attn.cuh"
 #include "combine.cuh"
-#include "common.cuh"
 #include "qknorm_rope.cuh"
 #include "sm90.cuh"
 
 #include <type_traits>
 
 namespace b200 {
-
-int get_tensor_map_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                      uint64_t row_stride_bytes, uint32_t box_cols, uint32_t box_rows, bool is_bf16);
-
 namespace dtc {
 
 using namespace sm90;
 
-constexpr int kD = 128;
+constexpr int kD = kHeadDim;
 constexpr int kTileN = 128;                 // keys per tile
 constexpr int kStages = 3;
 constexpr int kThreads = 320;
@@ -120,17 +115,17 @@ struct Unit {
 };
 static_assert(sizeof(Unit) <= 40, "Unit must fit its smem slot");
 
-// Work unit `pos` of the size-sorted order (metadata.cu): entry = r | chunk << 16 | n_chunks << 20,
-// the hkv heads of an item are adjacent positions (neighbouring CTAs stream the same token rows).
+// Work unit `pos` of the size-sorted order (metadata.cu): the hkv heads of an item are adjacent positions
+// (neighbouring CTAs stream the same token rows).
 __device__ __forceinline__ Unit get_unit(int pos, int hkv, int chunk_tokens, const int32_t* order,
                                          const int32_t* seq_lens) {
   Unit u;
   const int item = pos / hkv;
   u.h = pos - item * hkv;
-  const int e = order[item];
-  u.r = e & 0xffff;
-  u.c = (e >> 16) & 0xf;
-  u.n_chunks = (e >> 20) & 0x1f;
+  const PlanEntry e = unpack_plan_entry(order[item]);
+  u.r = e.r;
+  u.c = e.c;
+  u.n_chunks = e.n_chunks;
   u.kv_len = seq_lens[u.r];
   u.kv_begin = u.c * chunk_tokens;
   const int kv_end = min(u.kv_len, u.kv_begin + chunk_tokens);
@@ -760,32 +755,42 @@ static int launch_g(const Params<T>& p, const CUtensorMap& mk, const CUtensorMap
 }
 
 template <typename T>
-static int launch(const Params<T>& p, cudaStream_t st) {
-  CUtensorMap mk, mv;
-  const bool bf16 = std::is_same<T, __nv_bfloat16>::value;
-  const uint64_t cols = (uint64_t)p.hkv * kD;
-  if (int rc = get_tensor_map_2d(&mk, p.k_cache, p.num_slots, cols, cols * 2, 64, 1, bf16)) return rc;
-  if (int rc = get_tensor_map_2d(&mv, p.v_cache, p.num_slots, cols, cols * 2, 64, 1, bf16)) return rc;
-  CUtensorMap bk = mk, bv = mv;
-  if (p.box_rows > 0) {
-    if (int rc = get_tensor_map_2d(&bk, p.k_cache, p.num_slots, cols, cols * 2, 64, p.box_rows, bf16)) return rc;
-    if (int rc = get_tensor_map_2d(&bv, p.v_cache, p.num_slots, cols, cols * 2, 64, p.box_rows, bf16)) return rc;
+static int launch(const DecodeArgs& a) {
+  // A batch the plan policy leaves unsplit needs no combine pass: run the in-kernel merge (a no-op
+  // then; still correct for a foreign plan that does split) and skip the combine launch.
+  int fused = g_decode_fused_combine.load();
+  if (fused == 2) fused = decode_plan_is_unsplit(a.bs, a.hkv, 2 * num_sms()) ? 1 : 0;
+  // K/V streaming ahead of the predecessor: only for launches that are being captured into a graph
+  int early = 0;
+  if (g_decode_early_kv.load()) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(a.stream, &cs) == cudaSuccess && cs == cudaStreamCaptureStatusActive) early = 1;
   }
+  const DecodeWorkspace ws = carve_decode_workspace(a.workspace, a.workspace_bytes, a.bs, a.hq);
+  const Params<T> p{(const T*)a.q, a.q_rs, (const T*)a.k, a.k_rs, (const T*)a.v, a.v_rs, (T*)a.k_cache,
+                    (T*)a.v_cache, a.out_loc, a.slot_table, a.st_stride, a.seq_lens, a.plan, a.bs, a.hq, a.hkv,
+                    (int)a.num_slots, box_rows_for(a.page_size), g_decode_exact_tail.load() ? 1 : 0, fused,
+                    a.scale * kLog2e, (T*)a.out, ws.part_o, ws.part_ml, ws.counters, early, a.fuse,
+                    (const T*)a.qw, (const T*)a.kw, a.eps, a.positions, a.cos_sin};
+  const bool bf16 = std::is_same<T, __nv_bfloat16>::value;
+  CUtensorMap mk, mv;
+  if (int rc = kv_pool_maps(&mk, &mv, a.k_cache, a.v_cache, a.num_slots, a.hkv, 1, bf16)) return rc;
+  CUtensorMap bk = mk, bv = mv;
+  if (p.box_rows > 0)
+    if (int rc = kv_pool_maps(&bk, &bv, a.k_cache, a.v_cache, a.num_slots, a.hkv, p.box_rows, bf16)) return rc;
   // 8-row boxes for the last page piece of a range (exact tail)
   CUtensorMap tk = bk, tv = bv;
-  if (p.box_rows > 8) {
-    if (int rc = get_tensor_map_2d(&tk, p.k_cache, p.num_slots, cols, cols * 2, 64, 8, bf16)) return rc;
-    if (int rc = get_tensor_map_2d(&tv, p.v_cache, p.num_slots, cols, cols * 2, 64, 8, bf16)) return rc;
-  }
+  if (p.box_rows > 8)
+    if (int rc = kv_pool_maps(&tk, &tv, a.k_cache, a.v_cache, a.num_slots, a.hkv, 8, bf16)) return rc;
   switch (p.hq / p.hkv) {
-    case 1: return launch_g<T, 1>(p, mk, mv, bk, bv, tk, tv, st);
-    case 2: return launch_g<T, 2>(p, mk, mv, bk, bv, tk, tv, st);
-    case 3: return launch_g<T, 3>(p, mk, mv, bk, bv, tk, tv, st);
-    case 4: return launch_g<T, 4>(p, mk, mv, bk, bv, tk, tv, st);
-    case 5: return launch_g<T, 5>(p, mk, mv, bk, bv, tk, tv, st);
-    case 6: return launch_g<T, 6>(p, mk, mv, bk, bv, tk, tv, st);
-    case 7: return launch_g<T, 7>(p, mk, mv, bk, bv, tk, tv, st);
-    case 8: return launch_g<T, 8>(p, mk, mv, bk, bv, tk, tv, st);
+    case 1: return launch_g<T, 1>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 2: return launch_g<T, 2>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 3: return launch_g<T, 3>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 4: return launch_g<T, 4>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 5: return launch_g<T, 5>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 6: return launch_g<T, 6>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 7: return launch_g<T, 7>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 8: return launch_g<T, 8>(p, mk, mv, bk, bv, tk, tv, a.stream);
     default:
       set_error("attn_decode: GQA group size %d not supported (1..8)", p.hq / p.hkv);
       return 1;
@@ -794,52 +799,75 @@ static int launch(const Params<T>& p, cudaStream_t st) {
 
 }  // namespace dtc
 
-extern std::atomic<int> g_decode_fused_combine;
-extern std::atomic<int> g_decode_early_kv;
-extern std::atomic<int> g_decode_exact_tail;
-bool decode_plan_is_unsplit(int bs, int num_kv_heads, int ctas);  // metadata.cu
-
-// entry used by b200_attn_decode (attn_decode.cu)
-int launch_decode_tc(const void* q, int64_t q_rs, const void* k, int64_t k_rs, const void* v,
-                     int64_t v_rs, void* k_cache, void* v_cache, const int32_t* out_loc,
-                     const int32_t* slot_table, int64_t st_stride, const int32_t* seq_lens,
-                     const int32_t* plan, int bs, int hq, int hkv, int64_t num_slots, int page_size,
-                     float scale_log2, void* out, float* part_o, float* part_ml, int* counters,
-                     int dtype, cudaStream_t st, int fuse, const void* qw, const void* kw, float eps,
-                     const int32_t* positions, const float* cos_sin) {
-  // A batch the plan policy leaves unsplit needs no combine pass: run the in-kernel merge (a no-op
-  // then; still correct for a foreign plan that does split) and skip the combine launch.
-  int fused = g_decode_fused_combine.load();
-  if (fused == 2) fused = decode_plan_is_unsplit(bs, hkv, 2 * num_sms()) ? 1 : 0;
-  // rows per tiled TMA box: largest power of two <= min(page_size, 64) that divides page_size
-  int box_rows = 0;
-  if (page_size >= 8) {
-    box_rows = 64;
-    while (box_rows > 8 && (page_size % box_rows) != 0) box_rows >>= 1;
-    if (page_size % box_rows != 0) box_rows = 0;
+// Every argument check of both decode entry points, then the kernel the options select.
+static int attn_decode(const DecodeArgs& a) {
+  if (a.fuse) {
+    B200_CHECK_ARG(a.positions != nullptr && a.cos_sin != nullptr,
+                   "attn_decode_fused: positions / cos_sin_cache must not be NULL");
+    B200_CHECK_ARG(((uintptr_t)a.qw % 16) == 0 && ((uintptr_t)a.kw % 16) == 0 && ((uintptr_t)a.cos_sin % 16) == 0,
+                   "attn_decode_fused: weights / cos_sin_cache must be 16-byte aligned");
   }
-  B200_CHECK_ARG(num_slots > 0 && num_slots < (1ll << 31), "attn_decode: bad num_slots %lld",
-                 (long long)num_slots);
-  // K/V streaming ahead of the predecessor: only for launches that are being captured into a graph
-  int early = 0;
-  if (g_decode_early_kv.load()) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    if (cudaStreamIsCapturing(st, &cs) == cudaSuccess && cs == cudaStreamCaptureStatusActive) early = 1;
-  }
-  B200_CHECK_ARG(st_stride % 4 == 0 && ((uintptr_t)slot_table % 16) == 0,
+  B200_CHECK_ARG(a.head_dim == kHeadDim, "attn_decode: head_dim must be 128 (got %d)", a.head_dim);
+  B200_CHECK_ARG(a.bs > 0 && a.hq > 0 && a.hkv > 0 && a.hq % a.hkv == 0, "attn_decode: bad bs/hq/hkv %d/%d/%d",
+                 a.bs, a.hq, a.hkv);
+  B200_CHECK_ARG(a.q_rs % 8 == 0 && a.k_rs % 8 == 0 && a.v_rs % 8 == 0,
+                 "attn_decode: row strides must be multiples of 8 elements");
+  B200_CHECK_ARG(((uintptr_t)a.q % 16) == 0 && ((uintptr_t)a.k % 16) == 0 && ((uintptr_t)a.v % 16) == 0 &&
+                     ((uintptr_t)a.k_cache % 16) == 0 && ((uintptr_t)a.v_cache % 16) == 0 &&
+                     ((uintptr_t)a.out % 16) == 0,
+                 "attn_decode: pointers must be 16-byte aligned");
+  const size_t ws_need = decode_workspace_bytes(a.bs, a.hq, a.head_dim);
+  B200_CHECK_ARG(a.workspace_bytes >= ws_need, "attn_decode: workspace too small (%zu < %zu)", a.workspace_bytes,
+                 ws_need);
+  B200_CHECK_ARG(a.plan != nullptr, "attn_decode: decode_plan is NULL (b200_build_metadata)");
+  B200_CHECK_ARG(a.page_size >= 1, "attn_decode: page_size must be >= 1");
+  B200_CHECK_ARG(a.dtype == B200_DTYPE_BF16 || a.dtype == B200_DTYPE_FP16, "attn_decode: bad dtype %d", a.dtype);
+  B200_CHECK_ARG(a.num_slots > 0 && a.num_slots < (1ll << 31), "attn_decode: bad num_slots %lld",
+                 (long long)a.num_slots);
+  B200_CHECK_ARG(a.st_stride % 4 == 0 && ((uintptr_t)a.slot_table % 16) == 0,
                  "attn_decode: slot table rows must be 16-byte aligned");
-#define RUN(T_)                                                                                   \
-  dtc::Params<T_> p{(const T_*)q, q_rs, (const T_*)k, k_rs, (const T_*)v, v_rs, (T_*)k_cache,     \
-                    (T_*)v_cache, out_loc, slot_table, st_stride, seq_lens, plan, bs, hq, hkv,    \
-                    (int)num_slots, box_rows, g_decode_exact_tail.load() ? 1 : 0, fused, scale_log2, \
-                    (T_*)out,                                                                     \
-                    part_o, part_ml, counters, early, fuse, (const T_*)qw, (const T_*)kw, eps, positions, cos_sin};  \
-  return dtc::launch<T_>(p, st)
-  if (dtype == B200_DTYPE_BF16) {
-    RUN(__nv_bfloat16);
-  }
-  RUN(__half);
-#undef RUN
+  if (g_decode_impl.load() == 1)
+    return a.dtype == B200_DTYPE_BF16 ? dtc::launch<__nv_bfloat16>(a) : dtc::launch<__half>(a);
+  B200_CHECK_ARG(!a.fuse, "attn_decode_fused: only the wgmma kernel (decode_impl = 1) fuses qk-norm + RoPE");
+#ifdef B200_BRINGUP_KERNELS
+  return launch_decode_bringup(a);
+#else
+  set_error("attn_decode: decode_impl = 0 (cp.async bring-up kernel) is not part of this build (B200_BUILD_BRINGUP=1)");
+  return 1;
+#endif
 }
 
 }  // namespace b200
+
+using namespace b200;
+
+extern "C" size_t b200_attn_workspace_bytes(int max_bs, int hq, int head_dim) {
+  return decode_workspace_bytes(max_bs, hq, head_dim);
+}
+
+extern "C" int b200_attn_decode(const void* q, int64_t q_row_stride, const void* k, int64_t k_row_stride,
+                                const void* v, int64_t v_row_stride, void* k_cache, void* v_cache,
+                                int64_t num_slots, int page_size, const int32_t* out_loc,
+                                const int32_t* slot_table, int64_t slot_table_stride, const int32_t* seq_lens,
+                                const int32_t* decode_plan, int bs, int hq, int hkv, int head_dim, float scale,
+                                void* out, void* workspace, size_t workspace_bytes, int dtype, void* stream) {
+  return attn_decode({q, q_row_stride, k, k_row_stride, v, v_row_stride, k_cache, v_cache, num_slots, page_size,
+                      out_loc, slot_table, slot_table_stride, seq_lens, decode_plan, bs, hq, hkv, head_dim, scale,
+                      out, workspace, workspace_bytes, dtype, (cudaStream_t)stream});
+}
+
+extern "C" int b200_attn_decode_fused(const void* q, int64_t q_row_stride, const void* k,
+                                      int64_t k_row_stride, const void* v, int64_t v_row_stride,
+                                      const void* q_weight, const void* k_weight, float eps,
+                                      const int32_t* positions, const float* cos_sin_cache,
+                                      void* k_cache, void* v_cache, int64_t num_slots, int page_size,
+                                      const int32_t* out_loc, const int32_t* slot_table,
+                                      int64_t slot_table_stride, const int32_t* seq_lens,
+                                      const int32_t* decode_plan, int bs, int hq, int hkv, int head_dim,
+                                      float scale, void* out, void* workspace, size_t workspace_bytes,
+                                      int dtype, void* stream) {
+  return attn_decode({q, q_row_stride, k, k_row_stride, v, v_row_stride, k_cache, v_cache, num_slots, page_size,
+                      out_loc, slot_table, slot_table_stride, seq_lens, decode_plan, bs, hq, hkv, head_dim, scale,
+                      out, workspace, workspace_bytes, dtype, (cudaStream_t)stream, 1, q_weight, k_weight, eps,
+                      positions, cos_sin_cache});
+}

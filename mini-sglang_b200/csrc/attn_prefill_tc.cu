@@ -18,22 +18,17 @@
 //               online softmax on the score fragments: a query row lives in one quad of lanes, so the row
 //               max / sum need two shuffles; K/V tiles that are fully masked for all 64 rows are skipped.
 // The producer warpgroup hands registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 = 384 x 168.
-#include "b200attn.h"
-#include "common.cuh"
+#include "attn.cuh"
 #include "sm90.cuh"
 
 #include <type_traits>
 
 namespace b200 {
-
-int get_tensor_map_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols,
-                      uint64_t row_stride_bytes, uint32_t box_cols, uint32_t box_rows, bool is_bf16);
-
 namespace ptc {
 
 using namespace sm90;
 
-constexpr int kD = 128;
+constexpr int kD = kHeadDim;
 constexpr int kBM = 128;                   // query rows per unit (two consumer warpgroups x 64)
 constexpr int kBN = 128;                   // keys per tile
 constexpr int kStages = 2;                 // K ring depth = V ring depth
@@ -88,9 +83,9 @@ __device__ __forceinline__ Unit get_unit(int pos, int hq, int group, const int32
   u.head = pos - item * hq;
   u.h = u.head / group;
   u.owner = (u.head == u.h * group);  // the first query head of a kv head appends its rows
-  const int e = items[item];
-  u.r = e & 0xffff;
-  u.q_start = ((e >> 16) & 0xffff) * kBM;
+  const int32_t e = items[item];
+  u.r = prefill_item_request(e);
+  u.q_start = prefill_item_q_tile(e) * kBM;
   u.q_begin = cu_q[u.r];
   u.q_len = cu_q[u.r + 1] - u.q_begin;
   u.kv_len = seq_lens[u.r];
@@ -482,30 +477,26 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
 }
 
 template <typename T>
-static int launch(const Params<T>& p, const void* q, int64_t q_rs, int64_t nnz, const void* k_cache,
-                  const void* v_cache, cudaStream_t st) {
-  CUtensorMap nk, nv, nbk, nbv;
+static int launch(const PrefillArgs& a) {
+  const Params<T> p{a.slot_table, a.st_stride, a.seq_lens, a.cu_q, a.plan, a.bs, a.hq, a.hkv, (int)a.num_slots,
+                    box_rows_for(a.page_size), a.scale * kLog2e, (T*)a.out, (const T*)a.k, (const T*)a.v, a.k_rs,
+                    (T*)a.k_cache, (T*)a.v_cache, a.out_loc, a.nnz, g_prefill_skip_append.load()};
   const bool bf16 = std::is_same<T, __nv_bfloat16>::value;
-  CUtensorMap mq, mk, mv, bk, bv;
   const uint64_t cols = (uint64_t)p.hkv * kD;
-  if (int rc = encode_tensor_map_2d(&mq, q, nnz, (uint64_t)p.hq * kD, q_rs * 2, 64, kBM, bf16)) return rc;
-  if (int rc = get_tensor_map_2d(&mk, k_cache, p.num_slots, cols, cols * 2, 64, 1, bf16)) return rc;
-  if (int rc = get_tensor_map_2d(&mv, v_cache, p.num_slots, cols, cols * 2, 64, 1, bf16)) return rc;
-  bk = mk;
-  bv = mv;
-  if (p.box_rows > 0) {
-    if (int rc = get_tensor_map_2d(&bk, k_cache, p.num_slots, cols, cols * 2, 64, p.box_rows, bf16)) return rc;
-    if (int rc = get_tensor_map_2d(&bv, v_cache, p.num_slots, cols, cols * 2, 64, p.box_rows, bf16)) return rc;
-  }
+  CUtensorMap mq, mk, mv, nk, nv;
+  if (int rc = encode_tensor_map_2d(&mq, a.q, a.nnz, (uint64_t)p.hq * kD, a.q_rs * 2, 64, kBM, bf16)) return rc;
+  if (int rc = kv_pool_maps(&mk, &mv, a.k_cache, a.v_cache, a.num_slots, a.hkv, 1, bf16)) return rc;
+  CUtensorMap bk = mk, bv = mv;
+  if (p.box_rows > 0)
+    if (int rc = kv_pool_maps(&bk, &bv, a.k_cache, a.v_cache, a.num_slots, a.hkv, p.box_rows, bf16)) return rc;
   // the k / v inputs of this forward as [nnz, hkv*128] row-strided tensors (not cached: activations
   // move between forwards)
-  if (int rc = encode_tensor_map_2d(&nk, p.k_new, nnz, cols, p.kv_rs * 2, 64, 1, bf16)) return rc;
-  if (int rc = encode_tensor_map_2d(&nv, p.v_new, nnz, cols, p.kv_rs * 2, 64, 1, bf16)) return rc;
-  nbk = nk;
-  nbv = nv;
+  if (int rc = encode_tensor_map_2d(&nk, p.k_new, a.nnz, cols, p.kv_rs * 2, 64, 1, bf16)) return rc;
+  if (int rc = encode_tensor_map_2d(&nv, p.v_new, a.nnz, cols, p.kv_rs * 2, 64, 1, bf16)) return rc;
+  CUtensorMap nbk = nk, nbv = nv;
   if (p.box_rows > 0) {
-    if (int rc = encode_tensor_map_2d(&nbk, p.k_new, nnz, cols, p.kv_rs * 2, 64, p.box_rows, bf16)) return rc;
-    if (int rc = encode_tensor_map_2d(&nbv, p.v_new, nnz, cols, p.kv_rs * 2, 64, p.box_rows, bf16)) return rc;
+    if (int rc = encode_tensor_map_2d(&nbk, p.k_new, a.nnz, cols, p.kv_rs * 2, 64, p.box_rows, bf16)) return rc;
+    if (int rc = encode_tensor_map_2d(&nbv, p.v_new, a.nnz, cols, p.kv_rs * 2, 64, p.box_rows, bf16)) return rc;
   }
   const size_t smem = Smem::total + 1024;
   static bool configured = false;
@@ -514,41 +505,53 @@ static int launch(const Params<T>& p, const void* q, int64_t q_rs, int64_t nnz, 
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  attn_prefill_tc_kernel<T><<<num_sms(), kThreads, smem, st>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
+  attn_prefill_tc_kernel<T><<<num_sms(), kThreads, smem, a.stream>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
   B200_POST_LAUNCH();
   return 0;
 }
 
 }  // namespace ptc
 
-extern std::atomic<int> g_prefill_skip_append;
-
-// entry used by b200_attn_prefill (attn_prefill.cu)
-int launch_prefill_tc(const void* q, int64_t q_rs, int64_t nnz, const void* k, const void* v, int64_t kv_rs,
-                      void* k_cache, void* v_cache, const int32_t* out_loc, const int32_t* slot_table, int64_t st_stride, const int32_t* seq_lens,
-                      const int32_t* cu_q, const int32_t* prefill_plan, int bs, int hq, int hkv,
-                      int64_t num_slots, int page_size, float scale_log2, void* out, int dtype,
-                      cudaStream_t st) {
-  B200_CHECK_ARG(num_slots > 0 && num_slots < (1ll << 31), "attn_prefill: bad num_slots");
-  B200_CHECK_ARG(st_stride % 4 == 0 && ((uintptr_t)slot_table % 16) == 0,
+// Every argument check of b200_attn_prefill, then the kernel the plan and the options select.
+static int attn_prefill(const PrefillArgs& a) {
+  B200_CHECK_ARG(a.head_dim == kHeadDim, "attn_prefill: head_dim must be 128 (got %d)", a.head_dim);
+  B200_CHECK_ARG(a.bs > 0 && a.hq > 0 && a.hkv > 0 && a.hq % a.hkv == 0, "attn_prefill: bad bs/hq/hkv %d/%d/%d",
+                 a.bs, a.hq, a.hkv);
+  B200_CHECK_ARG(a.max_q >= 1 && a.nnz >= a.bs, "attn_prefill: bad max_seqlen_q/nnz");
+  B200_CHECK_ARG(a.q_rs % 8 == 0 && a.k_rs % 8 == 0 && a.v_rs % 8 == 0,
+                 "attn_prefill: row strides must be multiples of 8 elements");
+  B200_CHECK_ARG(a.k_rs == a.v_rs, "attn_prefill: k and v must share a row stride");
+  B200_CHECK_ARG(((uintptr_t)a.q % 16) == 0 && ((uintptr_t)a.k % 16) == 0 && ((uintptr_t)a.v % 16) == 0 &&
+                     ((uintptr_t)a.k_cache % 16) == 0 && ((uintptr_t)a.v_cache % 16) == 0 &&
+                     ((uintptr_t)a.out % 16) == 0,
+                 "attn_prefill: pointers must be 16-byte aligned");
+  B200_CHECK_ARG(a.dtype == B200_DTYPE_BF16 || a.dtype == B200_DTYPE_FP16, "attn_prefill: bad dtype %d", a.dtype);
+  B200_CHECK_ARG(a.num_slots > 0 && a.num_slots < (1ll << 31), "attn_prefill: bad num_slots");
+  B200_CHECK_ARG(a.st_stride % 4 == 0 && ((uintptr_t)a.slot_table % 16) == 0,
                  "attn_prefill: slot table rows must be 16-byte aligned");
-  B200_CHECK_ARG(prefill_plan != nullptr, "attn_prefill: prefill_plan is NULL (b200_build_prefill_plan)");
-  int box_rows = 0;
-  if (page_size >= 8) {
-    box_rows = 64;
-    while (box_rows > 8 && (page_size % box_rows) != 0) box_rows >>= 1;
-    if (page_size % box_rows != 0) box_rows = 0;
-  }
-#define RUN(T_)                                                                                    \
-  ptc::Params<T_> p{slot_table, st_stride, seq_lens, cu_q, prefill_plan, bs, hq, hkv, (int)num_slots, \
-                    box_rows, scale_log2, (T_*)out, (const T_*)k, (const T_*)v, kv_rs, (T_*)k_cache,  \
-                    (T_*)v_cache, out_loc, nnz, g_prefill_skip_append.load()};                                                   \
-  return ptc::launch<T_>(p, q, q_rs, nnz, k_cache, v_cache, st)
-  if (dtype == B200_DTYPE_BF16) {
-    RUN(__nv_bfloat16);
-  }
-  RUN(__half);
-#undef RUN
+  if (a.plan != nullptr && g_prefill_impl.load() == 1 && a.hq / a.hkv <= 16)  // append fused
+    return a.dtype == B200_DTYPE_BF16 ? ptc::launch<__nv_bfloat16>(a) : ptc::launch<__half>(a);
+#ifdef B200_BRINGUP_KERNELS
+  return launch_prefill_bringup(a);
+#else
+  set_error("attn_prefill: needs a prefill_plan (b200_build_prefill_plan) and a GQA group <= 16; the mma.sync bring-up kernel "
+            "(prefill_impl = 0) is not part of this build (B200_BUILD_BRINGUP=1)");
+  return 1;
+#endif
 }
 
 }  // namespace b200
+
+extern "C" int b200_attn_prefill(const void* q, int64_t q_row_stride, const void* k, int64_t k_row_stride,
+                                 const void* v, int64_t v_row_stride, void* k_cache, void* v_cache,
+                                 int64_t num_slots, int page_size, const int32_t* out_loc, const int32_t* slot_table,
+                                 int64_t slot_table_stride, const int32_t* seq_lens, const int32_t* cu_seqlens_q,
+                                 const int32_t* prefill_plan, int bs, int64_t nnz, int max_seqlen_q, int hq, int hkv,
+                                 int head_dim, float scale, void* out, void* workspace, size_t workspace_bytes,
+                                 int dtype, void* stream) {
+  (void)workspace;
+  (void)workspace_bytes;
+  return b200::attn_prefill({q, q_row_stride, k, k_row_stride, v, v_row_stride, k_cache, v_cache, num_slots,
+                             page_size, out_loc, slot_table, slot_table_stride, seq_lens, cu_seqlens_q, prefill_plan,
+                             bs, nnz, max_seqlen_q, hq, hkv, head_dim, scale, out, dtype, (cudaStream_t)stream});
+}

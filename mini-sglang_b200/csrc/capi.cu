@@ -36,7 +36,23 @@ std::atomic<int> g_decode_plan_nosplit{75};  // no split once bs * kv_heads * 10
 std::atomic<int> g_decode_fused_combine{1};
 std::atomic<int> g_decode_early_kv{1};  // captured decode launches stream K/V without waiting for the predecessor
 std::atomic<int> g_decode_exact_tail{1};  // box mode: the last page piece of a range loads only its valid rows
-}
+
+static const struct {
+  const char* name;
+  std::atomic<int>* value;
+} kOptions[] = {
+    {"use_pdl", &g_use_pdl},
+    {"decode_impl", &g_decode_impl},
+    {"prefill_skip_append", &g_prefill_skip_append},
+    {"prefill_order", &g_prefill_order},
+    {"prefill_impl", &g_prefill_impl},
+    {"decode_plan_target", &g_decode_plan_target},
+    {"decode_plan_nosplit", &g_decode_plan_nosplit},
+    {"decode_early_kv", &g_decode_early_kv},
+    {"decode_fused_combine", &g_decode_fused_combine},
+    {"decode_exact_tail", &g_decode_exact_tail},
+};
+}  // namespace b200
 
 extern "C" int b200_abi_version(void) { return 7; }
 
@@ -47,21 +63,13 @@ extern "C" int b200_abi_version(void) { return 7; }
 extern "C" const char* b200_build_digest(void) { return B200_BUILD_DIGEST + 11; }
 
 extern "C" int b200_set_option(const char* name, int value) {
+  if (name == nullptr) return -1;
 #ifndef B200_BRINGUP_KERNELS
   // the cross-check kernels are compiled into test builds only (B200_BUILD_BRINGUP=1)
-  if (name != nullptr && value == 0 && (std::strcmp(name, "decode_impl") == 0 || std::strcmp(name, "prefill_impl") == 0))
-    return -1;
+  if (value == 0 && (std::strcmp(name, "decode_impl") == 0 || std::strcmp(name, "prefill_impl") == 0)) return -1;
 #endif
-  if (name != nullptr && std::strcmp(name, "use_pdl") == 0) return b200::g_use_pdl.exchange(value);
-  if (name != nullptr && std::strcmp(name, "decode_impl") == 0) return b200::g_decode_impl.exchange(value);
-  if (name != nullptr && std::strcmp(name, "prefill_skip_append") == 0) return b200::g_prefill_skip_append.exchange(value);
-  if (name != nullptr && std::strcmp(name, "prefill_order") == 0) return b200::g_prefill_order.exchange(value);
-  if (name != nullptr && std::strcmp(name, "prefill_impl") == 0) return b200::g_prefill_impl.exchange(value);
-  if (name != nullptr && std::strcmp(name, "decode_plan_target") == 0) return b200::g_decode_plan_target.exchange(value);
-  if (name != nullptr && std::strcmp(name, "decode_plan_nosplit") == 0) return b200::g_decode_plan_nosplit.exchange(value);
-  if (name != nullptr && std::strcmp(name, "decode_early_kv") == 0) return b200::g_decode_early_kv.exchange(value);
-  if (name != nullptr && std::strcmp(name, "decode_fused_combine") == 0) return b200::g_decode_fused_combine.exchange(value);
-  if (name != nullptr && std::strcmp(name, "decode_exact_tail") == 0) return b200::g_decode_exact_tail.exchange(value);
+  for (const auto& o : b200::kOptions)
+    if (std::strcmp(name, o.name) == 0) return o.value->exchange(value);
   return -1;
 }
 

@@ -1,13 +1,9 @@
 // Split-KV combine shared by the decode kernels: merges the per-chunk partial (o, m, l) written by
 // the attention kernel into the final output (flash-decoding reduction).
 #pragma once
-#include "common.cuh"
+#include "attn.cuh"
 
 namespace b200 {
-
-constexpr int kPlanHeader = 4;   // decode_plan = {chunk_tokens, total_chunks, bs, 0, chunk_start[bs+1]}
-constexpr int kMaxSplits = 16;   // chunks per request (metadata.cu guarantees the bound)
-constexpr int kHeadDim = 128;
 
 // ------------------------------------------------------------------------------- combine
 // grid (bs, hq), 128 threads (one per output dim). Requests with a single chunk were already

@@ -56,7 +56,17 @@ inline int num_sms() {
   return cached;
 }
 
+// b200_set_option knobs (defined, with their defaults, in capi.cu; include/b200attn.h documents them)
 extern std::atomic<int> g_use_pdl;
+extern std::atomic<int> g_decode_impl;
+extern std::atomic<int> g_prefill_impl;
+extern std::atomic<int> g_prefill_order;
+extern std::atomic<int> g_prefill_skip_append;
+extern std::atomic<int> g_decode_plan_target;
+extern std::atomic<int> g_decode_plan_nosplit;
+extern std::atomic<int> g_decode_fused_combine;
+extern std::atomic<int> g_decode_early_kv;
+extern std::atomic<int> g_decode_exact_tail;
 
 // kernel<<<grid, block, smem, stream>>>(args...) with the programmatic-stream-serialization attribute
 template <typename... KArgs, typename... Args>
@@ -172,6 +182,12 @@ __device__ __forceinline__ void stg_stream(void* p, const Vec8& v) {
 // cp.async 16 B global -> shared (LDGSTS), L2-only caching
 __device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void* gptr) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr), "l"(gptr)
+               : "memory");
+}
+// as cp_async16, but !valid writes 16 zero bytes and reads nothing
+__device__ __forceinline__ void cp_async16_zfill(uint32_t smem_addr, const void* gptr, bool valid) {
+  const int sz = valid ? 16 : 0;
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_addr), "l"(gptr), "r"(sz)
                : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }

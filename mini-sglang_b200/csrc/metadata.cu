@@ -3,13 +3,10 @@
 // triples (table_idx, cached_len, device_len) into seq_lens / cu_seqlens_q / cu_seqlens_k,
 // a token-granular slot-table snapshot (one row per request) and the split-KV decode plan.
 // Integer work only -- results must be bit-identical to the reference's host arithmetic.
-#include "b200attn.h"
-#include "common.cuh"
+#include "attn.cuh"
 
 namespace b200 {
 
-constexpr int kPlanHeader = 4;  // {chunk_tokens, total_chunks, bs, reserved}
-constexpr int kMaxSplits = 16;  // chunks per request never exceed this (workspace sizing)
 constexpr int kOrderBins = 128; // counting-sort bins (tiles per work item, clamped)
 
 // ---- row snapshot: slot_table[r][0:width] = page_table[table_idx_r][0:width]
@@ -133,7 +130,6 @@ __global__ void __launch_bounds__(1024) meta_scan_kernel(const int32_t* __restri
   // ---- work order: (request, chunk) items sorted by size, largest first (counting sort on the
   // number of 128-token tiles).  The decode kernel deals them to its persistent CTAs in snake
   // order, which balances the per-CTA work to within about one tile.
-  // entry = r | chunk_idx << 16 | n_chunks << 20   (r < 65536, chunk_idx < 16, n_chunks <= 16)
   __shared__ int hist[kOrderBins];
   for (int i = tid; i < kOrderBins; i += 1024) hist[i] = 0;
   __syncthreads();
@@ -164,14 +160,13 @@ __global__ void __launch_bounds__(1024) meta_scan_kernel(const int32_t* __restri
     const int nc = (kl + chunk - 1) / chunk;
     for (int c = 0; c < nc; ++c) {
       const int pos = atomicAdd(&hist[tiles_of(kl, nc, c)], 1);
-      order[pos] = r | (c << 16) | (nc << 20);
+      order[pos] = pack_plan_entry(r, c, nc);
     }
   }
 }
 
 // ---- prefill plan: (request, 128-row q tile) items, heaviest (most KV tiles under the causal mask)
 // first; the prefill kernel deals them to its persistent CTAs in snake order.
-// plan = {n_items, 0, 0, 0, item[...]},  item = r | q_tile << 16
 constexpr int kPrefillBins = 1024;
 __global__ void __launch_bounds__(1024) meta_prefill_plan_kernel(const int32_t* __restrict__ req_info,
                                                                  int bs, int32_t* __restrict__ plan,
@@ -192,7 +187,7 @@ __global__ void __launch_bounds__(1024) meta_prefill_plan_kernel(const int32_t* 
       const int incl = block_scan_incl(nq, sm, &tot);
       const int start = carry + incl - nq;
       if (r < bs && carry + tot <= capacity)
-        for (int qt = 0; qt < nq; ++qt) plan[4 + start + (nq - 1 - qt)] = r | (qt << 16);
+        for (int qt = 0; qt < nq; ++qt) plan[4 + start + (nq - 1 - qt)] = pack_prefill_item(r, qt);
       carry += tot;
     }
     if (tid == 0) {
@@ -234,18 +229,13 @@ __global__ void __launch_bounds__(1024) meta_prefill_plan_kernel(const int32_t* 
     const int nq = (kl - cached + 127) / 128;
     for (int qt = 0; qt < nq; ++qt) {
       const int pos = atomicAdd(&hist[work_of(cached, kl, qt)], 1);
-      plan[4 + pos] = r | (qt << 16);
+      plan[4 + pos] = pack_prefill_item(r, qt);
     }
   }
 }
 
 }  // namespace b200
 
-namespace b200 {
-extern std::atomic<int> g_prefill_order;
-extern std::atomic<int> g_decode_plan_target;
-extern std::atomic<int> g_decode_plan_nosplit;
-}
 using namespace b200;
 
 extern "C" int b200_build_prefill_plan(const int32_t* req_info, int bs, int32_t* prefill_plan,

@@ -1,7 +1,7 @@
 // Host side of TMA: tensor-map encoding through the driver entry point (resolved at run time via
 // the CUDA runtime, so libb200attn.so does not link against libcuda) and a small cache keyed by
 // (base pointer, shape) -- the KV pool layers are the only tensors ever described.
-#include "common.cuh"
+#include "attn.cuh"
 #include "sm90.cuh"
 
 #include <cudaTypedefs.h>

@@ -2,6 +2,7 @@
 mirrored onto the GPU for the product path."""
 from __future__ import annotations
 
+import contextlib
 import importlib
 import random
 from dataclasses import dataclass
@@ -9,10 +10,29 @@ from types import SimpleNamespace
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
+import pytest
 import torch
 
 from oracle import attention as o_attn
 from oracle import metadata as o_meta
+
+
+@contextlib.contextmanager
+def options(b200, **opts):
+    """Sets b200_set_option knobs for the duration of the block, then restores their previous values.  Skips the
+    test when a knob is refused: the bring-up kernels (decode_impl / prefill_impl = 0) are only in
+    B200_BUILD_BRINGUP=1 builds."""
+    prev = []
+    try:
+        for name, val in opts.items():
+            try:
+                prev.append((name, b200._cabi.set_option(name, val)))
+            except b200._cabi.B200NativeError:
+                pytest.skip(f"option {name}={val}: cross-check kernel not in this build (B200_BUILD_BRINGUP=1)")
+        yield
+    finally:
+        for name, val in reversed(prev):
+            b200._cabi.set_option(name, val)
 
 
 @dataclass

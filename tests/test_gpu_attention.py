@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GpuWorld, add_requests, attn_tolerance_ok, make_inputs, make_world, oracle_forward
+from helpers import GpuWorld, add_requests, attn_tolerance_ok, make_inputs, make_world, options, oracle_forward
 from oracle import metadata as o_meta
 
 pytestmark = pytest.mark.gpu
@@ -20,14 +20,8 @@ def decode_impl(request, b200, native_lib):
     the "in kernel only when nothing is split" policy, and the cp.async / CUDA-core bring-up kernel
     (selected with the debug options)."""
     impl = 0 if request.param == 0 else 1
-    try:
-        prev = b200._cabi.set_option("decode_impl", impl)
-    except b200._cabi.B200NativeError:
-        pytest.skip("cross-check kernel not in this build (B200_BUILD_BRINGUP=1)")
-    prev_merge = b200._cabi.set_option("decode_fused_combine", {3: 2, 2: 0}.get(request.param, 1))
-    yield impl
-    b200._cabi.set_option("decode_impl", prev)
-    b200._cabi.set_option("decode_fused_combine", prev_merge)
+    with options(b200, decode_impl=impl, decode_fused_combine={3: 2, 2: 0}.get(request.param, 1)):
+        yield impl
 
 
 def _check_metadata(md, ref: o_meta.RefMetadata, page_size: int):
@@ -150,14 +144,8 @@ def prefill_impl(request, b200, native_lib):
     """The tensor-core product kernel (wgmma on sm_90a; the ids keep the variant names the suite has
     always used) with the request-major work order (option prefill_order = 1) and with the size-sorted
     order (default), and the mma.sync bring-up kernel (test builds only)."""
-    try:
-        prev = b200._cabi.set_option("prefill_impl", 0 if request.param == 0 else 1)
-    except b200._cabi.B200NativeError:
-        pytest.skip("cross-check kernel not in this build (B200_BUILD_BRINGUP=1)")
-    prev_order = b200._cabi.set_option("prefill_order", 1 if request.param == 1 else 0)
-    yield request.param
-    b200._cabi.set_option("prefill_impl", prev)
-    b200._cabi.set_option("prefill_order", prev_order)
+    with options(b200, prefill_impl=0 if request.param == 0 else 1, prefill_order=1 if request.param == 1 else 0):
+        yield request.param
 
 
 PREFILL_LENS = {

@@ -6,7 +6,6 @@ names the position and kv head the kernel attended to instead.  Ramps (prefill):
 own position (rising) or key 0 (falling).  Regimes: peaked, flat, drifting and chunk-offset softmaxes against
 the fp64 reference's element-wise bound.  Every pool row no request owns, and every slot this forward appends
 to, is NaN before the launch."""
-import contextlib
 import math
 import random
 
@@ -14,7 +13,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GpuWorld, World, add_requests
+from helpers import GpuWorld, World, add_requests, options
 from oracle import metadata as o_meta
 from oracle import probes as P
 
@@ -33,21 +32,6 @@ def _tail_lens(page_size):
     while page_size % rb:
         rb >>= 1
     return sorted({k * page_size + r + 1 for k in (2, 5) for r in (0, 1, 7, 8, 9, rb - 1, page_size - 1)})
-
-
-@contextlib.contextmanager
-def _options(b200, opts):
-    prev = []
-    try:
-        for name, val in opts.items():
-            try:
-                prev.append((name, b200._cabi.set_option(name, val)))
-            except b200._cabi.B200NativeError:
-                pytest.skip(f"option {name}={val}: cross-check kernel not in this build (B200_BUILD_BRINGUP=1)")
-        yield
-    finally:
-        for name, val in reversed(prev):
-            b200._cabi.set_option(name, val)
 
 
 def _decode_opts(plan, merge=1, impl=1):
@@ -88,7 +72,7 @@ def _run(b200, w, phase, build, opts, world=None):
     batch = gw.batch(phase)
     batch.out_loc = torch.from_numpy(md.out_loc).cuda()
     batch.positions = torch.from_numpy(md.positions).cuda()
-    with _options(b200, opts):
+    with options(b200, **opts):
         gw.backend.prepare_metadata(batch)
         chunk = int(batch.attn_metadata.decode_plan[0])
         assert chunk % 128 == 0

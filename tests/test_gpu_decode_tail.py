@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GpuWorld, add_requests, attn_tolerance_ok, make_inputs, make_world, oracle_forward
+from helpers import GpuWorld, add_requests, attn_tolerance_ok, make_inputs, make_world, options, oracle_forward
 from oracle import metadata as o_meta
 
 pytestmark = pytest.mark.gpu
@@ -26,64 +26,63 @@ def _box_rows(page_size):
 
 
 def _run_arm(b200, w, ref_md, qkv, exact, mode, pad_to, pre):
-    prev = b200._cabi.set_option("decode_exact_tail", exact)
-    try:
-        gw = GpuWorld(b200, w)
-        backend = gw.backend
-        x = qkv.cuda()
-        bs = x.shape[0]
-        positions = torch.from_numpy(ref_md.positions).cuda()
-        out_loc = torch.from_numpy(ref_md.out_loc).cuda()
-        if mode == "graph":
-            # captured like the engine's decode graphs: the K/V producers start before the predecessor finishes
-            backend.init_capture_graph(w.page_table.shape[1], [bs])
-            dummy = b200.Req(table_idx=w.page_table.shape[0] - 1, cached_len=0, device_len=1)
-            qkv_buf = torch.zeros_like(x)
-            pos_buf = torch.zeros(bs, dtype=torch.int32, device="cuda")
-            loc_buf = torch.full((bs,), int(w.page_table[-1, 0]), dtype=torch.int32, device="cuda")
-            out_buf = torch.zeros(bs, HQ, D, dtype=x.dtype, device="cuda")
-            cap = b200.Batch([dummy] * bs, "decode")
-            cap.padded_reqs = cap.reqs
-            backend.prepare_for_capture(cap)
-            cap.out_loc, cap.positions = loc_buf, pos_buf
+    with options(b200, decode_exact_tail=exact):
+        try:
+            gw = GpuWorld(b200, w)
+            backend = gw.backend
+            x = qkv.cuda()
+            bs = x.shape[0]
+            positions = torch.from_numpy(ref_md.positions).cuda()
+            out_loc = torch.from_numpy(ref_md.out_loc).cuda()
+            if mode == "graph":
+                # captured like the engine's decode graphs: the K/V producers start before the predecessor finishes
+                backend.init_capture_graph(w.page_table.shape[1], [bs])
+                dummy = b200.Req(table_idx=w.page_table.shape[0] - 1, cached_len=0, device_len=1)
+                qkv_buf = torch.zeros_like(x)
+                pos_buf = torch.zeros(bs, dtype=torch.int32, device="cuda")
+                loc_buf = torch.full((bs,), int(w.page_table[-1, 0]), dtype=torch.int32, device="cuda")
+                out_buf = torch.zeros(bs, HQ, D, dtype=x.dtype, device="cuda")
+                cap = b200.Batch([dummy] * bs, "decode")
+                cap.padded_reqs = cap.reqs
+                backend.prepare_for_capture(cap)
+                cap.out_loc, cap.positions = loc_buf, pos_buf
 
-            def run():
-                q, k, v = qkv_buf.split([HQ * D, HKV * D, HKV * D], dim=-1)
-                out_buf.copy_(backend.forward_decode_fused(q.view(-1, HQ, D), k, v, 0, cap, pos_buf, *pre))
+                def run():
+                    q, k, v = qkv_buf.split([HQ * D, HKV * D, HKV * D], dim=-1)
+                    out_buf.copy_(backend.forward_decode_fused(q.view(-1, HQ, D), k, v, 0, cap, pos_buf, *pre))
 
-            stream = torch.cuda.Stream()
-            with torch.cuda.stream(stream):
-                run()
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph, stream=stream):
+                stream = torch.cuda.Stream()
+                with torch.cuda.stream(stream):
                     run()
-            torch.cuda.synchronize()
-            batch = gw.batch("decode", pad_to=pad_to)
-            batch.out_loc, batch.positions = out_loc, positions
-            backend.prepare_metadata(batch)
-            with torch.cuda.stream(stream):
-                qkv_buf.copy_(x)
-                pos_buf.copy_(positions)
-                loc_buf.copy_(out_loc)
-                backend.prepare_for_replay(batch)
-                graph.replay()
-            out = out_buf
-        else:
-            batch = gw.batch("decode", pad_to=pad_to)
-            batch.out_loc, batch.positions = out_loc, positions
-            backend.prepare_metadata(batch)
-            q, k, v = x.split([HQ * D, HKV * D, HKV * D], dim=-1)
-            if mode == "fused":
-                out = backend.forward_decode_fused(q.view(-1, HQ, D), k, v, 0, batch, positions, *pre)
+                    graph = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(graph, stream=stream):
+                        run()
+                torch.cuda.synchronize()
+                batch = gw.batch("decode", pad_to=pad_to)
+                batch.out_loc, batch.positions = out_loc, positions
+                backend.prepare_metadata(batch)
+                with torch.cuda.stream(stream):
+                    qkv_buf.copy_(x)
+                    pos_buf.copy_(positions)
+                    loc_buf.copy_(out_loc)
+                    backend.prepare_for_replay(batch)
+                    graph.replay()
+                out = out_buf
             else:
-                out = backend.forward(q.view(-1, HQ, D), k, v, 0, batch)
-        torch.cuda.synchronize()
-        plan = batch.attn_metadata.decode_plan.cpu()
-        kc, vc = gw.pool_rows(0)
-        return out.cpu(), kc, vc, plan
-    finally:
-        b200._cabi.set_option("decode_exact_tail", prev)
-        b200.core.set_global_ctx(None)
+                batch = gw.batch("decode", pad_to=pad_to)
+                batch.out_loc, batch.positions = out_loc, positions
+                backend.prepare_metadata(batch)
+                q, k, v = x.split([HQ * D, HKV * D, HKV * D], dim=-1)
+                if mode == "fused":
+                    out = backend.forward_decode_fused(q.view(-1, HQ, D), k, v, 0, batch, positions, *pre)
+                else:
+                    out = backend.forward(q.view(-1, HQ, D), k, v, 0, batch)
+            torch.cuda.synchronize()
+            plan = batch.attn_metadata.decode_plan.cpu()
+            kc, vc = gw.pool_rows(0)
+            return out.cpu(), kc, vc, plan
+        finally:
+            b200.core.set_global_ctx(None)
 
 
 def _check(b200, *, page_size, lens, mode="eager", pad_to=None, force_split=False, seed=0):
@@ -116,13 +115,8 @@ def _check(b200, *, page_size, lens, mode="eager", pad_to=None, force_split=Fals
     w.reqs = saved
 
     # force_split: split every request into 128-key chunks (as many items as the policy allows)
-    prev = [(name, b200._cabi.set_option(name, val)) for name, val in
-            (("decode_plan_nosplit", 0), ("decode_plan_target", 16))] if force_split else []
-    try:
+    with options(b200, **({"decode_plan_nosplit": 0, "decode_plan_target": 16} if force_split else {})):
         (o1, k1, v1, plan), (o0, k0, v0, _) = [_run_arm(b200, w, ref_md, qkv, arm, mode, pad_to, pre) for arm in (1, 0)]
-    finally:
-        for name, val in prev:
-            b200._cabi.set_option(name, val)
     assert torch.equal(o1[:n_real].view(torch.int16), o0[:n_real].view(torch.int16)), \
         f"outputs differ: max |d| {(o1[:n_real].float() - o0[:n_real].float()).abs().max().item():.3e}"
     # the whole pool, except the slot the padding requests all append to (many writers)

@@ -34,8 +34,8 @@ TAIL_BOX = 8  # rows of the boxes the piece holding the end of a range is loaded
 
 
 def box_rows_for(page_size: int) -> int:
-    """Rows per tiled TMA box at this page size (launch_decode_tc): the largest power of two <= min(page size, 64)
-    that divides the page size, 0 = row mode (page sizes below 8)."""
+    """Rows per tiled TMA box at this page size (box_rows_for in csrc/attn.cuh): the largest power of two
+    <= min(page size, 64) that divides the page size, 0 = row mode (page sizes below 8)."""
     if page_size < 8:
         return 0
     rb = 64
