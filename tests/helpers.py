@@ -35,6 +35,10 @@ def options(b200, **opts):
             b200._cabi.set_option(name, val)
 
 
+# options(b200, **SPLIT_PLAN): every decode request split into 128-key chunks, as many as the plan allows
+SPLIT_PLAN = {"decode_plan_nosplit": 0, "decode_plan_target": 16}
+
+
 @dataclass
 class World:
     page_size: int
@@ -98,10 +102,26 @@ def add_requests(w: World, lens: Sequence[Tuple[int, int]], share_prefix_from: O
         w.reqs.append((t, c, dl))
 
 
-def make_inputs(w: World, seed: int, strided: bool = True):
-    """q/k/v for the new tokens as row-strided views of one qkv buffer (layers/attention.py:49)."""
+def padded_reqs(w: World, pad_to: Optional[int] = None) -> List[Tuple[int, int, int]]:
+    """w.reqs followed by dummy requests up to pad_to, as a graph-padded batch has them (GpuWorld.batch): the
+    page table's last row, kv_len 1, all appending to the dummy page's first slot."""
+    return list(w.reqs) + [(w.page_table.shape[0] - 1, 0, 1)] * ((pad_to or 0) - len(w.reqs))
+
+
+def poison_unowned(w: World) -> None:
+    """NaN in every CPU pool row no request owns, before GpuWorld mirrors the pool: unused page tails and free
+    pages hold arbitrary bits in a real engine (torch.empty pool) and must never leak into a result."""
+    used = np.zeros(w.pool_cpu.shape[2], dtype=bool)
+    for (t, _, d) in w.reqs:
+        used[w.page_table[t, :d]] = True
+    w.pool_cpu[:, :, torch.from_numpy(~used)] = float("nan")
+
+
+def make_inputs(w: World, seed: int, strided: bool = True, reqs: Optional[Sequence[Tuple[int, int, int]]] = None):
+    """q/k/v for the new tokens of `reqs` (default w.reqs) as row-strided views of one qkv buffer
+    (layers/attention.py:49)."""
     g = torch.Generator().manual_seed(seed)
-    nnz = sum(d - c for (_, c, d) in w.reqs)
+    nnz = sum(d - c for (_, c, d) in (w.reqs if reqs is None else reqs))
     width = (w.hq + 2 * w.hkv) * w.d
     qkv = torch.randn((nnz, width), generator=g, dtype=torch.float32).to(w.dtype)
     if not strided:
@@ -111,13 +131,15 @@ def make_inputs(w: World, seed: int, strided: bool = True):
     return qkv, q, k, v
 
 
-def oracle_forward(w: World, layer: int, q, k, v, md: o_meta.RefMetadata, fp32: bool = True):
-    """Runs store + attention on CPU copies; returns (out, k_cache_after, v_cache_after)."""
+def oracle_forward(w: World, layer: int, q, k, v, md: o_meta.RefMetadata, fp32: bool = True,
+                   reqs: Optional[Sequence[Tuple[int, int, int]]] = None):
+    """Runs store + attention of `reqs` (default w.reqs) on CPU copies; returns (out, k_cache_after, v_cache_after)."""
+    reqs = w.reqs if reqs is None else reqs
     kc = w.pool_cpu[0, layer].clone()
     vc = w.pool_cpu[1, layer].clone()
     nnz = q.shape[0]
-    rows = [torch.from_numpy(md.slot_table[i, : md.cache_seqlens[i]].copy()) for i in range(len(w.reqs))]
-    q_lens = [d - c for (_, c, d) in w.reqs]
+    rows = [torch.from_numpy(md.slot_table[i, : md.cache_seqlens[i]].copy()) for i in range(len(reqs))]
+    q_lens = [d - c for (_, c, d) in reqs]
     from oracle.store import ref_store_kv
 
     ref_store_kv(kc, vc, torch.from_numpy(md.out_loc.copy()), k.reshape(nnz, -1), v.reshape(nnz, -1))
@@ -146,6 +168,30 @@ def attn_tolerance_ok(ours: torch.Tensor, ref32: torch.Tensor, what: str = ""):
     return rel_fro
 
 
+def assert_bits_equal(a: torch.Tensor, b: torch.Tensor, what: str):
+    """a and b (16-bit, on any device) hold the same bits; a failure reports the largest difference."""
+    a, b = a.cpu(), b.cpu()
+    assert a.shape == b.shape, f"{what}: shapes {tuple(a.shape)} vs {tuple(b.shape)}"
+    assert torch.equal(a.view(torch.int16), b.view(torch.int16)), \
+        f"{what}: bits differ, max |a - b| {(a.float() - b.float()).abs().max().item():.3e}"
+
+
+def box_rows(page_size: int) -> int:
+    """Rows per tiled TMA box of the decode K/V loads (box_rows_for in csrc/attn.cuh): the largest power of two
+    from 8 to 64 that divides the page size, 0 = row mode."""
+    rows = 64
+    while rows > 8 and page_size % rows:
+        rows >>= 1
+    return rows if page_size % rows == 0 else 0
+
+
+def tail_range_ends(page_size: int) -> List[int]:
+    """Streamed range lengths n (kv_len - 1) whose end falls at every offset of interest in the last page of a
+    box-mode page size (>= 8): n mod page_size in {0, 1, 7, 8, 9, box_rows - 1, page_size - 1}, sorted."""
+    rb = box_rows(page_size)
+    return sorted({k * page_size + r for k in (2, 5) for r in (0, 1, 7, 8, 9, rb - 1, page_size - 1)})
+
+
 class GpuWorld:
     """Device-side mirror of a World wired into the product's Context / pool / backend."""
 
@@ -164,16 +210,86 @@ class GpuWorld:
         ctx.attn_backend = self.backend
         self.ctx, self.pool, self.dev = ctx, pool, dev
 
-    def batch(self, phase: str, pad_to: Optional[int] = None):
+    def batch(self, phase: str, pad_to: Optional[int] = None, md: Optional[o_meta.RefMetadata] = None):
+        """A batch of w.reqs, padded with dummy requests to pad_to; md: out_loc and positions from the oracle's
+        metadata of the padded requests."""
         b200 = self.b200
         reqs = [b200.Req(table_idx=t, cached_len=c, device_len=d) for (t, c, d) in self.w.reqs]
         batch = b200.Batch(reqs, phase)
         if pad_to is not None and pad_to > len(reqs):
             dummy = b200.Req(table_idx=self.w.page_table.shape[0] - 1, cached_len=0, device_len=1)
             batch.padded_reqs = reqs + [dummy] * (pad_to - len(reqs))
+        if md is not None:
+            batch.out_loc = torch.from_numpy(md.out_loc).to(self.dev)
+            batch.positions = torch.from_numpy(md.positions).to(self.dev)
         return batch
 
     def pool_rows(self, layer: int):
-        kc = self.pool.k_cache(layer).reshape(-1, self.w.hkv, self.w.d).cpu()
-        vc = self.pool.v_cache(layer).reshape(-1, self.w.hkv, self.w.d).cpu()
+        """K and V rows [slots, hkv, d] of one pool layer, on the device."""
+        kc = self.pool.k_cache(layer).reshape(-1, self.w.hkv, self.w.d)
+        vc = self.pool.v_cache(layer).reshape(-1, self.w.hkv, self.w.d)
         return kc, vc
+
+
+def run_attention(gw: GpuWorld, batch, qkv: torch.Tensor, *, layer: int = 0, fused: Optional[tuple] = None,
+                  graph: bool = False, prepare: bool = True):
+    """One attention launch of `batch` on the device rows `qkv` [nnz, (hq + 2 hkv) d], as the engine runs it:
+    prepare_metadata (unless the caller ran it already: prepare=False), then `forward`, or for a decode batch
+    with fused = (cos_sin_cache, q_weight, k_weight, eps) `forward_decode_fused` on the raw q / k rows.  graph:
+    the decode launch is captured into a CUDA graph on a dummy batch of the same size and replayed on `batch`
+    after prepare_for_replay, like the engine's graph runner.  Synchronises.  Returns (out, decode plan, pool K
+    rows, pool V rows of the layer), all on the device."""
+    w, backend = gw.w, gw.backend
+
+    def launch(x, b):
+        q, k, v = x.split([w.hq * w.d, w.hkv * w.d, w.hkv * w.d], dim=-1)
+        if fused is None:
+            return backend.forward(q.view(-1, w.hq, w.d), k, v, layer, b)
+        return backend.forward_decode_fused(q.view(-1, w.hq, w.d), k, v, layer, b, b.positions, *fused)
+
+    if not graph:
+        if prepare:
+            backend.prepare_metadata(batch)
+        out = launch(qkv, batch)
+    else:
+        # static buffers of the "graph runner", captured on a batch of dummy requests of the same size
+        bs = batch.padded_size
+        backend.init_capture_graph(w.page_table.shape[1], [bs])
+        dummy = gw.b200.Req(table_idx=w.page_table.shape[0] - 1, cached_len=0, device_len=1)
+        cap = gw.b200.Batch([dummy] * bs, "decode")
+        cap.padded_reqs = cap.reqs
+        backend.prepare_for_capture(cap)
+        qkv_buf = torch.zeros_like(qkv)
+        cap.positions = torch.zeros(bs, dtype=torch.int32, device=gw.dev)
+        cap.out_loc = torch.full((bs,), int(w.page_table[-1, 0]), dtype=torch.int32, device=gw.dev)
+        out = torch.zeros(bs, w.hq, w.d, dtype=qkv.dtype, device=gw.dev)
+        stream = torch.cuda.Stream()
+        with torch.cuda.stream(stream):
+            out.copy_(launch(qkv_buf, cap))  # warm-up outside the capture
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=stream):
+                out.copy_(launch(qkv_buf, cap))
+        torch.cuda.synchronize()
+        if prepare:
+            backend.prepare_metadata(batch)
+        stream.wait_stream(torch.cuda.current_stream())  # the live metadata is built on the current stream
+        with torch.cuda.stream(stream):
+            qkv_buf.copy_(qkv)
+            cap.positions.copy_(batch.positions)
+            cap.out_loc.copy_(batch.out_loc)
+            backend.prepare_for_replay(batch)
+            g.replay()
+    torch.cuda.synchronize()
+    return (out, batch.attn_metadata.decode_plan) + gw.pool_rows(layer)
+
+
+def replan(gw: GpuWorld, batch, num_ctas: int) -> None:
+    """Rebuilds the prepared metadata of `batch` in place, with the decode plan made for a grid of num_ctas CTAs
+    instead of the device's (a much larger grid splits every request into several chunks)."""
+    md, pt, b200 = batch.attn_metadata, gw.ctx.page_table, gw.b200
+    flat, _, _ = b200.attention.backend.host_req_info(batch.padded_reqs)
+    info = torch.tensor(flat, dtype=torch.int32, device=gw.dev)
+    b200._cabi.check(gw.backend._lib.b200_build_metadata(
+        info.data_ptr(), md.bs, pt.data_ptr(), pt.stride(0), md.cache_seqlens.data_ptr(), md.cu_seqlens_q.data_ptr(),
+        md.cu_seqlens_k.data_ptr(), md.page_table.data_ptr(), md.page_table.stride(0), md.page_table.shape[1],
+        md.decode_plan.data_ptr(), gw.w.hkv, num_ctas, torch.cuda.current_stream().cuda_stream), "b200_build_metadata")

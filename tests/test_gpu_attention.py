@@ -6,7 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GpuWorld, add_requests, attn_tolerance_ok, make_inputs, make_world, options, oracle_forward
+from helpers import (GpuWorld, add_requests, assert_bits_equal, attn_tolerance_ok, make_inputs, make_world, options,
+                     oracle_forward, padded_reqs, poison_unowned, replan, run_attention)
 from oracle import metadata as o_meta
 
 pytestmark = pytest.mark.gpu
@@ -63,47 +64,27 @@ def _run_case(b200, *, page_size, hq, hkv, lens, phase, seed=0, share_prefix=Non
     w = make_world(seed=seed, page_size=page_size, hq=hq, hkv=hkv, layers=layers,
                    max_reqs=max(len(lens), pad_to or 0) + 1, max_seq=max_seq, dtype=dtype)
     add_requests(w, lens, share_prefix_from=share_prefix)
-    # every pool row no request owns is poisoned with NaN: unused page tails / free pages hold
-    # arbitrary bits in a real engine (torch.empty pool) and must never leak into a result
-    used = np.zeros(w.pool_cpu.shape[2], dtype=bool)
-    for (t, _, d) in w.reqs:
-        used[w.page_table[t, :d]] = True
+    poison_unowned(w)
+    reqs = padded_reqs(w, pad_to)
+    ref_md = o_meta.ref_prepare_metadata(w.page_table, reqs, page_size)
+    qkv, q, k, v = make_inputs(w, seed + 1, reqs=reqs)
+    ref_out, ref_kc, ref_vc = oracle_forward(w, layer, q, k, v, ref_md, reqs=reqs)
     gw = GpuWorld(b200, w)
-    gw.pool._kv_buffer.view(2, w.layers, -1, hkv, w.d)[:, :, torch.from_numpy(~used).cuda()] = float("nan")
-    pool_before = gw.pool._kv_buffer.view(2, w.layers, -1, hkv, w.d)[0, layer].clone()
-    batch = gw.batch(phase, pad_to=pad_to)
-    triples = list(w.reqs)
-    if pad_to:
-        dummy_row = w.page_table.shape[0] - 1
-        triples += [(dummy_row, 0, 1)] * (pad_to - len(w.reqs))
-    ref_md = o_meta.ref_prepare_metadata(w.page_table, triples, page_size)
-    # inputs for all padded rows
-    w_full = w
-    saved = w.reqs
-    w.reqs = triples
-    qkv, q, k, v = make_inputs(w, seed + 1)
-    ref_out, ref_kc, ref_vc = oracle_forward(w, layer, q, k, v, ref_md)
-    w.reqs = saved
-    qkv_g = qkv.cuda()
-    qg, kg, vg = qkv_g.split([hq * w.d, hkv * w.d, hkv * w.d], dim=-1)
-    batch.positions = torch.from_numpy(ref_md.positions).cuda()
-    batch.out_loc = torch.from_numpy(ref_md.out_loc).cuda()
+    batch = gw.batch(phase, pad_to=pad_to, md=ref_md)
     gw.backend.prepare_metadata(batch)
     _check_metadata(batch.attn_metadata, ref_md, page_size)
-    out = gw.backend.forward(qg.view(-1, hq, w.d), kg, vg, layer, batch)
-    torch.cuda.synchronize()
+    out, _, kc, vc = run_attention(gw, batch, qkv.cuda(), layer=layer, prepare=False)
     assert out.shape == (qkv.shape[0], hq, w.d) and out.is_contiguous()
-    n_real = sum(d - c for (_, c, d) in saved)
+    n_real = sum(d - c for (_, c, d) in w.reqs)
     rel = attn_tolerance_ok(out[:n_real], ref_out[:n_real], f"{phase} ps={page_size} hq={hq} hkv={hkv}")
     # append side effect: pool rows bit-exact (dummy slot excluded: many writers)
-    kc, vc = gw.pool_rows(layer)
     real_slots = torch.from_numpy(ref_md.out_loc[:n_real].astype(np.int64))
-    assert torch.equal(kc[real_slots].view(torch.int16), ref_kc[real_slots].view(torch.int16))
-    assert torch.equal(vc[real_slots].view(torch.int16), ref_vc[real_slots].view(torch.int16))
-    # nothing else in the pool moved
+    assert_bits_equal(kc[real_slots], ref_kc[real_slots], "appended k rows")
+    assert_bits_equal(vc[real_slots], ref_vc[real_slots], "appended v rows")
+    # nothing else in the pool moved (the oracle's pool is the poisoned pool before the launch plus the appends)
     mask = torch.ones(kc.shape[0], dtype=torch.bool)
     mask[torch.from_numpy(ref_md.out_loc.astype(np.int64))] = False
-    assert torch.equal(kc[mask].view(torch.int16), pool_before.cpu()[mask].view(torch.int16))
+    assert_bits_equal(kc[mask], ref_kc[mask], "k rows nobody appended to")
     return rel
 
 
@@ -196,59 +177,20 @@ def test_forward_rejects_cpu_and_foreign_metadata(b200, native_lib):
 
 def test_cuda_graph_capture_and_replay(b200, native_lib, decode_impl):
     """init_capture_graph / prepare_for_capture / prepare_for_replay drive a captured decode
-    (reference engine/graph.py:105-158): replayed output == eager output, pool rows appended."""
-    hq, hkv, d, ps = 16, 8, 128, 16
-    lens = [(99, 100), (511, 512), (300, 301)]
-    w = make_world(seed=4, page_size=ps, hq=hq, hkv=hkv, max_reqs=9, max_seq=1024)
-    add_requests(w, lens)
+    (reference engine/graph.py:105-158) replayed on a live batch padded to the captured size: output
+    against the oracle, pool rows appended."""
+    ps = 16
+    w = make_world(seed=4, page_size=ps, hq=16, hkv=8, max_reqs=9, max_seq=1024)
+    add_requests(w, [(99, 100), (511, 512), (300, 301)])
+    reqs = padded_reqs(w, 4)
+    ref_md = o_meta.ref_prepare_metadata(w.page_table, reqs, ps)
+    qkv, q, k, v = make_inputs(w, 9, reqs=reqs)
+    ref_out, ref_kc, _ = oracle_forward(w, 0, q, k, v, ref_md, reqs=reqs)
     gw = GpuWorld(b200, w)
-    backend = gw.backend
-    max_seq_al = w.page_table.shape[1]
-    backend.init_capture_graph(max_seq_al, [4, 8])
-    dummy_row = w.page_table.shape[0] - 1
-    # static buffers owned by the "graph runner"
-    bs_cap = 4
-    qkv_buf = torch.zeros(bs_cap, (hq + 2 * hkv) * d, dtype=torch.bfloat16, device="cuda")
-    out_loc_buf = torch.zeros(bs_cap, dtype=torch.int32, device="cuda")
-    out_buf = torch.zeros(bs_cap, hq, d, dtype=torch.bfloat16, device="cuda")
-    cap_batch = b200.Batch([b200.Req(table_idx=dummy_row, cached_len=0, device_len=1)] * bs_cap, "decode")
-    cap_batch.padded_reqs = cap_batch.reqs
-    backend.prepare_for_capture(cap_batch)
-    cap_batch.out_loc = out_loc_buf
-    out_loc_buf.fill_(int(w.page_table[dummy_row, 0]))
-
-    def run():
-        q, k, v = qkv_buf.split([hq * d, hkv * d, hkv * d], dim=-1)
-        out_buf.copy_(backend.forward(q.view(-1, hq, d), k, v, 0, cap_batch))
-
-    stream = torch.cuda.Stream()
-    with torch.cuda.stream(stream):
-        run()  # warm-up outside capture
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=stream):
-            run()
-    torch.cuda.synchronize()
-
-    # live batch, padded to 4
-    batch = gw.batch("decode", pad_to=bs_cap)
-    triples = list(w.reqs) + [(dummy_row, 0, 1)]
-    ref_md = o_meta.ref_prepare_metadata(w.page_table, triples, ps)
-    saved, w.reqs = w.reqs, triples
-    qkv, q, k, v = make_inputs(w, 9)
-    ref_out, ref_kc, _ = oracle_forward(w, 0, q, k, v, ref_md)
-    w.reqs = saved
-    batch.out_loc = torch.from_numpy(ref_md.out_loc).cuda()
-    backend.prepare_metadata(batch)
-    with torch.cuda.stream(stream):
-        qkv_buf.copy_(qkv.cuda())
-        out_loc_buf.copy_(batch.out_loc)
-        backend.prepare_for_replay(batch)
-        graph.replay()
-    torch.cuda.synchronize()
-    attn_tolerance_ok(out_buf[:3], ref_out[:3], "graph replay")
-    kc, _ = gw.pool_rows(0)
+    out, _, kc, _ = run_attention(gw, gw.batch("decode", pad_to=4, md=ref_md), qkv.cuda(), graph=True)
+    attn_tolerance_ok(out[:3], ref_out[:3], "graph replay")
     slots = torch.from_numpy(ref_md.out_loc[:3].astype(np.int64))
-    assert torch.equal(kc[slots].view(torch.int16), ref_kc[slots].view(torch.int16))
+    assert_bits_equal(kc[slots], ref_kc[slots], "appended k rows")
 
 
 def test_decode_full_size_properties(b200, native_lib, decode_impl):
@@ -262,20 +204,16 @@ def test_decode_full_size_properties(b200, native_lib, decode_impl):
     w = make_world(seed=2, page_size=ps, hq=hq, hkv=hkv, max_reqs=bs, max_seq=2048)
     add_requests(w, lens)
     gw = GpuWorld(b200, w)
-    batch = gw.batch("decode")
     ref_md = o_meta.ref_prepare_metadata(w.page_table, w.reqs, ps)
     qkv, q, k, v = make_inputs(w, 3)
-    qkv_g = qkv.cuda()
-    qg, kg, vg = qkv_g.split([hq * d, hkv * d, hkv * d], dim=-1)
-    batch.out_loc = torch.from_numpy(ref_md.out_loc).cuda()
-    gw.backend.prepare_metadata(batch)
-    out = gw.backend.forward(qg.view(-1, hq, d), kg, vg, 0, batch).clone()
-    torch.cuda.synchronize()
+    batch = gw.batch("decode", md=ref_md)
+    x = qkv.cuda()
+    out, _, kc, vc = run_attention(gw, batch, x)
+    kc, vc = kc.cpu(), vc.cpu()  # copies: (d) scales the device pool
     # (a)
-    kc, vc = gw.pool_rows(0)
     slots = torch.from_numpy(ref_md.out_loc.astype(np.int64))
-    assert torch.equal(kc[slots].view(torch.int16), k.reshape(bs, hkv, d).contiguous().view(torch.int16))
-    assert torch.equal(vc[slots].view(torch.int16), v.reshape(bs, hkv, d).contiguous().view(torch.int16))
+    assert_bits_equal(kc[slots], k.reshape(bs, hkv, d), "appended k rows")
+    assert_bits_equal(vc[slots], v.reshape(bs, hkv, d), "appended v rows")
     # (b) sample
     from oracle.attention import ref_attention_one
     for r in rnd.sample(range(bs), 6):
@@ -285,22 +223,14 @@ def test_decode_full_size_properties(b200, native_lib, decode_impl):
         attn_tolerance_ok(out[r : r + 1], ref, f"sample req {r}")
     # (c) different chunking: the default plan keeps 256 requests unsplit; a plan built for a much
     # larger grid splits every request into several chunks (partials + combine)
-    md = batch.attn_metadata
-    lib = native_lib
-    info = torch.tensor([x for t in w.reqs for x in t], dtype=torch.int32).cuda()
-    rc = lib.b200_build_metadata(info.data_ptr(), bs, gw.ctx.page_table.data_ptr(), gw.ctx.page_table.stride(0),
-                                 md.cache_seqlens.data_ptr(), md.cu_seqlens_q.data_ptr(), md.cu_seqlens_k.data_ptr(),
-                                 md.page_table.data_ptr(), md.page_table.stride(0), md.page_table.shape[1],
-                                 md.decode_plan.data_ptr(), hkv, 8192, torch.cuda.current_stream().cuda_stream)
-    assert rc == 0
-    out2 = gw.backend.forward(qg.view(-1, hq, d), kg, vg, 0, batch)
-    torch.cuda.synchronize()
-    assert int(md.decode_plan[1]) > bs  # really split
+    replan(gw, batch, 8192)
+    out2, plan, _, _ = run_attention(gw, batch, x, prepare=False)
+    assert int(plan[1]) > bs  # really split
     assert (out2.float() - out.float()).abs().max().item() <= 2e-2 * out.float().abs().max().item()
     # (d) linearity in V: attn(V) with V scaled by 2 == 2 * attn(V) up to rounding
     gw.pool._kv_buffer[1].mul_(2)
-    out3 = gw.backend.forward(qg.view(-1, hq, d), kg, vg * 2, 0, batch)
-    torch.cuda.synchronize()
+    x[:, (hq + hkv) * d :] *= 2
+    out3, _, _, _ = run_attention(gw, batch, x, prepare=False)
     assert (out3.float() - 2 * out2.float()).abs().max().item() <= 2e-2 * out3.float().abs().max().item()
 
 
@@ -325,16 +255,11 @@ def test_attention_against_flashinfer_golden(b200, native_lib, phase):
     w = World(ps, num_pages, hq, hkv, d, 1, torch.bfloat16, pt.copy(), [], pool, reqs)
     md = o_meta.ref_prepare_metadata(pt, reqs, ps)
     gw = GpuWorld(b200, w)
-    batch = gw.batch(phase)
     loc = torch.from_numpy(md.out_loc.astype(np.int64))
-    q = bf(fi[f"{phase}_q"]).cuda()
-    k_new = pool[0, 0, loc].reshape(len(loc), -1).cuda()  # the golden pool already holds the appended rows
-    v_new = pool[1, 0, loc].reshape(len(loc), -1).cuda()
-    batch.out_loc = torch.from_numpy(md.out_loc).cuda()
-    batch.positions = torch.from_numpy(md.positions).cuda()
-    gw.backend.prepare_metadata(batch)
-    out = gw.backend.forward(q, k_new, v_new, 0, batch)
-    torch.cuda.synchronize()
+    q = bf(fi[f"{phase}_q"]).reshape(len(loc), -1)
+    # the golden pool already holds the appended rows
+    qkv = torch.cat([q, pool[0, 0, loc].reshape(len(loc), -1), pool[1, 0, loc].reshape(len(loc), -1)], 1)
+    out, _, _, _ = run_attention(gw, gw.batch(phase, md=md), qkv.cuda())
     want = bf(fi[f"{phase}_out"]).float()
     got = out.float().cpu()
     scale = want.abs().max().item()
@@ -364,53 +289,34 @@ def _fused_vs_unfused(b200, *, page_size, hq, hkv, lens, with_norm=True, pad_to=
     w = make_world(seed=seed, page_size=page_size, hq=hq, hkv=hkv, max_reqs=max(len(lens), pad_to or 0) + 1,
                    max_seq=max_seq, dtype=dtype)
     add_requests(w, lens)
-    triples = list(w.reqs)
-    if pad_to:
-        triples += [(w.page_table.shape[0] - 1, 0, 1)] * (pad_to - len(w.reqs))
-    ref_md = o_meta.ref_prepare_metadata(w.page_table, triples, page_size)
-    saved, w.reqs = w.reqs, triples
-    qkv, _, _, _ = make_inputs(w, seed + 1)
-    w.reqs = saved
+    reqs = padded_reqs(w, pad_to)
+    ref_md = o_meta.ref_prepare_metadata(w.page_table, reqs, page_size)
+    qkv, _, _, _ = make_inputs(w, seed + 1, reqs=reqs)
     d = w.d
     cache = ref_cos_sin_cache(d, max(4096, max_seq), 1e6).cuda()
     g = torch.Generator().manual_seed(seed)
     qw = (torch.rand(d, generator=g) + 0.5).to(dtype).cuda() if with_norm else None
     kw = (torch.rand(d, generator=g) + 0.5).to(dtype).cuda() if with_norm else None
-    prev = b200._cabi.set_option("decode_plan_nosplit", 0) if force_split else None
-    try:
-        results = []
-        for fused in (False, True):
-            gw = GpuWorld(b200, w)
-            batch = gw.batch("decode", pad_to=pad_to)
-            batch.positions = torch.from_numpy(ref_md.positions).cuda()
-            batch.out_loc = torch.from_numpy(ref_md.out_loc).cuda()
-            gw.backend.prepare_metadata(batch)
-            x = qkv.cuda()
-            q, k, v = x.split([hq * d, hkv * d, hkv * d], dim=-1)
-            if fused:
-                out = gw.backend.forward_decode_fused(q.view(-1, hq, d), k, v, 0, batch, batch.positions, cache, qw, kw, 1e-6)
-                torch.cuda.synchronize()
-                assert torch.equal(x.cpu().view(torch.int16), qkv.view(torch.int16)), "fused decode modified its raw inputs"
-            else:
-                b200.ops.qknorm_rope_inplace(batch.positions, q, k, d, cache, qw, kw, 1e-6)
-                out = gw.backend.forward(q.view(-1, hq, d), k, v, 0, batch)
-                torch.cuda.synchronize()
-            kc, vc = gw.pool_rows(0)
-            results.append((out.cpu(), kc, vc))
-            b200.core.set_global_ctx(None)
-    finally:
-        if prev is not None:
-            b200._cabi.set_option("decode_plan_nosplit", prev)
-    (o0, k0, v0), (o1, k1, v1) = results
+    with options(b200, **({"decode_plan_nosplit": 0} if force_split else {})):
+        gw = GpuWorld(b200, w)
+        batch = gw.batch("decode", pad_to=pad_to, md=ref_md)
+        gw.backend.prepare_metadata(batch)
+        x = qkv.cuda()
+        q, k, _ = x.split([hq * d, hkv * d, hkv * d], dim=-1)
+        b200.ops.qknorm_rope_inplace(batch.positions, q, k, d, cache, qw, kw, 1e-6)
+        o0, _, k0, v0 = run_attention(gw, batch, x, prepare=False)
+        gw = GpuWorld(b200, w)
+        x = qkv.cuda()
+        o1, _, k1, v1 = run_attention(gw, gw.batch("decode", pad_to=pad_to, md=ref_md), x, fused=(cache, qw, kw, 1e-6))
+        assert_bits_equal(x, qkv, "raw qkv rows after the fused decode")
     n_real = len(lens)
-    assert torch.equal(o0[:n_real].view(torch.int16), o1[:n_real].view(torch.int16)), \
-        f"fused output differs: max |d| {(o0[:n_real].float() - o1[:n_real].float()).abs().max().item():.3e}"
+    assert_bits_equal(o0[:n_real], o1[:n_real], "fused output")
     slots = torch.from_numpy(ref_md.out_loc[:n_real].astype(np.int64))
-    assert torch.equal(k0[slots].view(torch.int16), k1[slots].view(torch.int16))
-    assert torch.equal(v0[slots].view(torch.int16), v1[slots].view(torch.int16))
+    assert_bits_equal(k0[slots], k1[slots], "appended k rows")
+    assert_bits_equal(v0[slots], v1[slots], "appended v rows")
     mask = torch.ones(k0.shape[0], dtype=torch.bool)
     mask[torch.from_numpy(ref_md.out_loc.astype(np.int64))] = False
-    assert torch.equal(k0[mask].view(torch.int16), k1[mask].view(torch.int16))
+    assert_bits_equal(k0[mask], k1[mask], "k rows nobody appended to")
 
 
 @pytest.mark.parametrize("page_size", [1, 64])
@@ -476,16 +382,8 @@ def test_attention_against_reference_gpu_goldens(b200, native_lib, case):
 
     bf = lambda a: torch.from_numpy(a.view(np.int16).copy()).view(torch.bfloat16)  # noqa: E731
     w, md, qkv = build_case(case, helpers, o_meta)
-    hq, hkv, d = case["hq"], case["hkv"], 128
     gw = GpuWorld(b200, w)
-    batch = gw.batch(case["phase"])
-    g = qkv.cuda()
-    qg, kg, vg = g.split([hq * d, hkv * d, hkv * d], dim=-1)
-    batch.out_loc = torch.from_numpy(md.out_loc).cuda()
-    batch.positions = torch.from_numpy(md.positions).cuda()
-    gw.backend.prepare_metadata(batch)
-    out = gw.backend.forward(qg.view(-1, hq, d), kg, vg, 0, batch)
-    torch.cuda.synchronize()
+    out, _, _, _ = run_attention(gw, gw.batch(case["phase"], md=md), qkv.cuda())
     got = out[:: case["step"]].cpu()
     for ref_name in ("fi", "trtllm"):
         key = f"{case['name']}_{ref_name}"

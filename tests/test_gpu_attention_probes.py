@@ -13,7 +13,8 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GpuWorld, World, add_requests, options
+from helpers import (SPLIT_PLAN, GpuWorld, World, add_requests, assert_bits_equal, options, replan, run_attention,
+                     tail_range_ends)
 from oracle import metadata as o_meta
 from oracle import probes as P
 
@@ -27,19 +28,12 @@ GQA_SHAPES = [(16, 8), (8, 1), (40, 8), (64, 8), (7, 1), (6, 2)]
 DECODE_LENS = [1, 2, 3, 9, 129, 130, 257, 258, 385, 513, 1025, 2048]
 
 
-def _tail_lens(page_size):
-    rb = 64
-    while page_size % rb:
-        rb >>= 1
-    return sorted({k * page_size + r + 1 for k in (2, 5) for r in (0, 1, 7, 8, 9, rb - 1, page_size - 1)})
-
-
 def _decode_opts(plan, merge=1, impl=1):
     opts = {"decode_impl": impl, "decode_fused_combine": merge}
     if plan == "unsplit":
         opts["decode_plan_nosplit"] = 1
     else:
-        opts.update(decode_plan_nosplit=0, decode_plan_target=16)
+        opts.update(SPLIT_PLAN)
     return opts
 
 
@@ -62,34 +56,29 @@ def _world(*, page_size, hq, hkv, dtype, lens, num_pages=None, top=False, seed=0
     return w
 
 
-def _run(b200, w, phase, build, opts, world=None):
+def _run(b200, w, phase, build, opts):
     """prepare_metadata, then build(chunk) -> (kv, q) with kv = [(k [n, hkv, d], v [n, hkv, d])] per request
     (positions 0..n-1) and q [nnz, hq, d]; rows below cached_len go into the pool, the rest are this
     forward's k / v inputs.  Checks the appended pool rows bit for bit.  Returns (out, kv, q, gw, batch, qkv)."""
-    gw = world or GpuWorld(b200, w)
-    hq, hkv = w.hq, w.hkv
+    gw = GpuWorld(b200, w)
     md = o_meta.ref_prepare_metadata(w.page_table, w.reqs, w.page_size)
-    batch = gw.batch(phase)
-    batch.out_loc = torch.from_numpy(md.out_loc).cuda()
-    batch.positions = torch.from_numpy(md.positions).cuda()
+    batch = gw.batch(phase, md=md)
     with options(b200, **opts):
         gw.backend.prepare_metadata(batch)
         chunk = int(batch.attn_metadata.decode_plan[0])
         assert chunk % 128 == 0
         kv, q = build(chunk)
-        pool = gw.pool._kv_buffer.view(2, 1, -1, hkv, D)
+        pool = gw.pool_rows(0)
         idx = torch.cat([torch.from_numpy(w.page_table[t, :c].astype(np.int64)) for (t, c, _) in w.reqs]).cuda()
         for j in range(2):
-            pool[j, 0, idx] = torch.cat([x[j][:c] for x, (_, c, _) in zip(kv, w.reqs)]).cuda()
+            pool[j][idx] = torch.cat([x[j][:c] for x, (_, c, _) in zip(kv, w.reqs)]).cuda()
         new = [torch.cat([x[j][c:dl] for x, (_, c, dl) in zip(kv, w.reqs)]) for j in range(2)]
         nnz = q.shape[0]
         qkv = torch.cat([q.reshape(nnz, -1), new[0].reshape(nnz, -1), new[1].reshape(nnz, -1)], 1).cuda()
-        qg, kg, vg = qkv.split([hq * D, hkv * D, hkv * D], dim=-1)
-        out = gw.backend.forward(qg.view(nnz, hq, D), kg, vg, 0, batch)
-        torch.cuda.synchronize()
+        out, _, kc, vc = run_attention(gw, batch, qkv, prepare=False)
     slots = batch.out_loc.long()
-    for j in range(2):
-        assert torch.equal(pool[j, 0, slots].cpu().view(torch.int16), new[j].view(torch.int16)), "appended rows differ"
+    assert_bits_equal(kc[slots], new[0], "appended k rows")
+    assert_bits_equal(vc[slots], new[1], "appended v rows")
     return out.cpu(), kv, q, gw, batch, qkv
 
 
@@ -134,7 +123,7 @@ def _check_exact(out, want, kv, reqs, hq, hkv, what):
 
 
 def _decode_needles(b200, *, page_size, hq, hkv, dtype, plan, merge=1, impl=1, lens=None, ties=1, seed=0):
-    lens = lens or sorted(set(DECODE_LENS) | set(_tail_lens(page_size) if page_size >= 8 else []))
+    lens = lens or sorted(set(DECODE_LENS) | ({n + 1 for n in tail_range_ends(page_size)} if page_size >= 8 else set()))
     reqs = P.assign_needles(lens, page_size, hq, seed)
     w = _world(page_size=page_size, hq=hq, hkv=hkv, dtype=dtype, lens=[(n - 1, n) for n, _ in reqs], seed=seed)
     build, want = _decode_build(reqs, hq, hkv, dtype, seed, ties)
@@ -204,18 +193,10 @@ def test_decode_needles_full_size(b200, native_lib):
     out, kv, _, gw, batch, qkv = _run(b200, w, "decode", build, {})
     _check_exact(out, want, kv, reqs, hq, hkv, "full size, default plan")
     # re-plan for a much larger grid: every request split into several chunks (partials + merge)
-    md = batch.attn_metadata
-    info = torch.tensor([x for t in w.reqs for x in t], dtype=torch.int32).cuda()
-    rc = native_lib.b200_build_metadata(info.data_ptr(), len(reqs), gw.ctx.page_table.data_ptr(), gw.ctx.page_table.stride(0),
-                                        md.cache_seqlens.data_ptr(), md.cu_seqlens_q.data_ptr(), md.cu_seqlens_k.data_ptr(),
-                                        md.page_table.data_ptr(), md.page_table.stride(0), md.page_table.shape[1],
-                                        md.decode_plan.data_ptr(), hkv, 8192, torch.cuda.current_stream().cuda_stream)
-    assert rc == 0
+    replan(gw, batch, 8192)
     # the first forward appended the new rows: the pool now holds every key, the inputs stay the same
-    qg, kg, vg = qkv.split([hq * D, hkv * D, hkv * D], dim=-1)
-    out2 = gw.backend.forward(qg.view(-1, hq, D), kg, vg, 0, batch)
-    torch.cuda.synchronize()
-    assert int(md.decode_plan[1]) > len(reqs)
+    out2, plan, _, _ = run_attention(gw, batch, qkv, prepare=False)
+    assert int(plan[1]) > len(reqs)
     _check_exact(out2.cpu(), want, kv, reqs, hq, hkv, "full size, 8192-CTA plan")
 
 
@@ -223,7 +204,7 @@ def test_decode_needles_full_size(b200, native_lib):
 PREFILL_LENS = [(0, 200), (100, 300), (37, 200), (129, 400), (256, 700), (1, 140), (0, 1)]
 
 
-def _prefill_probe(b200, *, page_size, hq, hkv, dtype, lens, opts, seed=0, world=None, w=None):
+def _prefill_probe(b200, *, page_size, hq, hkv, dtype, lens, opts, seed=0, w=None):
     """Even query heads run needles (positions cached - 1, cached, cached + 127, cached + 128, the last key and
     a few more, one per head), odd heads ramps (rows with (i >> 3) & 1 == 0 rising, the others falling).  A row
     that sees its head's needle must return its V row exactly; a row before the needle must return the
@@ -259,7 +240,7 @@ def _prefill_probe(b200, *, page_size, hq, hkv, dtype, lens, opts, seed=0, world
             qs.append(q)
         return kv, torch.cat(qs).to(dtype)
 
-    out, kv, q, _, _, _ = _run(b200, w, "prefill", build, opts, world=world)
+    out, kv, q, _, _, _ = _run(b200, w, "prefill", build, opts)
     off, errors, worst = 0, [], 0.0
     for r, (_, c, dl) in enumerate(w.reqs):
         ql = dl - c
