@@ -1,11 +1,12 @@
 // The attention contract: what metadata.cu, the decode / prefill kernels and their entry points must agree on
-// (head dim, plan formats, decode workspace layout, TMA boxes over the KV pool) and the arguments an entry
-// point hands to a launcher.
+// (head dim, plan formats, decode workspace layout, TMA boxes over the KV pool), the arguments an entry
+// point hands to a launcher, and the device skeleton the two wgmma kernels share.
 #pragma once
 #include <cuda.h>
 
 #include "b200attn.h"
 #include "common.cuh"
+#include "sm90.cuh"
 
 namespace b200 {
 
@@ -109,6 +110,64 @@ int launch_prefill_bringup(const PrefillArgs& a);
 // Swizzled byte offset of 16-byte chunk c (0..15) of row `row` in a bring-up kernel's [rows][256 B] tile.
 __device__ __forceinline__ uint32_t swz(int row, int c) {
   return (uint32_t)(row * (kHeadDim * 2) + (((c & 8) | ((c ^ row) & 7)) << 4));
+}
+
+// ------------------------------------------------- device skeleton of the persistent wgmma kernels
+// Work dealing: the size-sorted units (metadata.cu) go to the persistent CTAs in snake order, the k-th unit of a
+// CTA being position k*grid + (k even ? cta : grid-1-cta), which balances per-CTA work to within about one unit.
+// Every role walks the same list: stage() decodes the first kCap units once, with the whole CTA, into smem
+// slots; at(k) reads them back, or decodes from global memory past the cap.  get(pos) is the kernel's decode.
+template <typename Unit, int kSlotBytes, int kCap, typename GetUnit>
+struct UnitList {
+  static_assert(sizeof(Unit) <= kSlotBytes, "Unit must fit its smem slot");
+  uint8_t* slots;
+  GetUnit get;
+  int total, n_rounds, grid, cta;
+  __device__ __forceinline__ static bool none(const Unit& u) { return u.n_tiles < 0; }  // no unit this round (the last)
+  __device__ __forceinline__ Unit decode(int k) const {
+    const int pos = k * grid + ((k & 1) ? grid - 1 - cta : cta);
+    Unit u;
+    u.n_tiles = -1;
+    if (pos < total) u = get(pos);
+    return u;
+  }
+  __device__ __forceinline__ void stage(int tid, int n_threads) const {
+    for (int k = tid; k < kCap && k < n_rounds; k += n_threads) *reinterpret_cast<Unit*>(slots + k * kSlotBytes) = decode(k);
+  }
+  __device__ __forceinline__ Unit at(int k) const {
+    return k < kCap ? *reinterpret_cast<const Unit*>(slots + k * kSlotBytes) : decode(k);
+  }
+};
+template <typename Unit, int kSlotBytes, int kCap, typename GetUnit>
+__device__ __forceinline__ UnitList<Unit, kSlotBytes, kCap, GetUnit> deal_units(uint8_t* slots, int total, GetUnit get) {
+  return {slots, get, total, (total + (int)gridDim.x - 1) / (int)gridDim.x, (int)gridDim.x, (int)blockIdx.x};
+}
+
+// K/V tile geometry: a K or V tile is 128 keys x 128 dims, two 64-column halves of [128 rows x 128 B], 128B-swizzled,
+// written in place by TMA.  A producer lane fills one half of a run of keys: in box mode (page_size >= 8) a box of
+// rb consecutive keys of one page, lane = (box, half); in row mode four keys, lane = (group, half) over the 16
+// groups of a part (part 0: keys 0-63, part 1: keys 64-127).
+constexpr int kKvTileRows = 128, kKvHalfBytes = kKvTileRows * 128, kKvTileBytes = 2 * kKvHalfBytes;
+struct KvLane {
+  int row, half;  // first key of the run within the tile, 64-column half
+  __device__ __forceinline__ static KvLane box(int lane, int rb) { return {(lane >> 1) * rb, lane & 1}; }
+  __device__ __forceinline__ static int box_lanes(int rb) { return (kKvTileRows / rb) * 2; }  // lanes with a box
+  __device__ __forceinline__ static KvLane group(int lane, int part) { return {(part * 16 + (lane >> 1)) * 4, lane & 1}; }
+  __device__ __forceinline__ uint32_t dst(uint32_t ring, uint32_t stage) const { return ring + stage * kKvTileBytes + half * kKvHalfBytes + row * 128; }
+  __device__ __forceinline__ int col(int col0) const { return col0 + half * 64; }
+};
+// Slots of keys pos0 .. pos0+3 (16-byte aligned); keys at or past `end` map to num_slots, out of range (zero filled).
+__device__ __forceinline__ int4 kv_slot_group(const int32_t* slots, int pos0, int end, int num_slots) {
+  if (pos0 + 3 < end) return __ldg(reinterpret_cast<const int4*>(slots + pos0));
+  auto slot = [&](int i) { return pos0 + i < end ? __ldg(slots + pos0 + i) : num_slots; };
+  return make_int4(slot(0), slot(1), slot(2), slot(3));
+}
+// the four single-row boxes of a row group
+__device__ __forceinline__ void tma_load_group(uint32_t dst, const CUtensorMap* m, uint32_t bar, int col, int4 rows) {
+  sm90::tma_load_2d(dst, m, bar, col, rows.x);
+  sm90::tma_load_2d(dst + 128, m, bar, col, rows.y);
+  sm90::tma_load_2d(dst + 256, m, bar, col, rows.z);
+  sm90::tma_load_2d(dst + 384, m, bar, col, rows.w);
 }
 
 }  // namespace b200

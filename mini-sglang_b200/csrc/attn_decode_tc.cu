@@ -35,7 +35,6 @@
 #include "attn.cuh"
 #include "combine.cuh"
 #include "qknorm_rope.cuh"
-#include "sm90.cuh"
 
 #include <type_traits>
 
@@ -45,29 +44,26 @@ namespace dtc {
 using namespace sm90;
 
 constexpr int kD = kHeadDim;
-constexpr int kTileN = 128;                 // keys per tile
 constexpr int kStages = 3;
 constexpr int kThreads = 320;
 constexpr int kWarpQ = 8, kWarpCombine = 9;
-constexpr int kHalfBytes = kTileN * 128;    // one 64-column half of a K or V tile: 16 KB
-constexpr int kStageBytes = 2 * kHalfBytes; // one K (or V) tile: half 0 | half 1 = 32 KB
 constexpr int kNPad = 8;                    // wgmma N (query heads of the group, padded)
 constexpr int kQBufBytes = 2 * 1024;        // two halves of [8 rows x 128 B], 128B-swizzled
-constexpr int kPBufBytes = kNPad * kTileN * 2;  // P^T [8 x 128] 16-bit, no-swizzle K-major
-constexpr int kMaxUnitsSmem = 96;           // per-CTA work units decoded once into smem
+constexpr int kPBufBytes = kNPad * kKvTileRows * 2;  // P^T [8 x 128] 16-bit, no-swizzle K-major
+constexpr int kUnitSlotBytes = 40, kMaxUnitsSmem = 96;  // per-CTA work units decoded once into smem
 constexpr int kEpiSlots = 4;                // fused mode: roped (q heads, new k) rows in flight to the epilogue
 constexpr int kEpiSlotBytes = 9 * kD * 2;   // up to 8 q heads + the k row, 128 x 16-bit each
 
 struct Smem {
   // offsets from the 1024-aligned base
   static constexpr int kring = 0;                          // K tiles, released right after QK
-  static constexpr int vring = kStages * kStageBytes;      // V tiles, released after PV
-  static constexpr int qbuf = 2 * kStages * kStageBytes;
+  static constexpr int vring = kStages * kKvTileBytes;     // V tiles, released after PV
+  static constexpr int qbuf = 2 * kStages * kKvTileBytes;
   static constexpr int pbuf = qbuf + 2 * kQBufBytes;
   static constexpr int bars = pbuf + kPBufBytes;           // 32 mbarriers
   static constexpr int red = bars + 32 * 8;                // floats: tile max [4][8], [2][4][8] row sums, [2][4][8] new-token dots
   static constexpr int units = red + (32 + 64 + 64) * 4;   // decoded work units
-  static constexpr int epi = units + kMaxUnitsSmem * 40;   // fused mode: kEpiSlots x [9][128] 16-bit
+  static constexpr int epi = units + kMaxUnitsSmem * kUnitSlotBytes;  // fused mode: kEpiSlots x [9][128] 16-bit
   static constexpr int total = epi + kEpiSlots * kEpiSlotBytes;
 };
 static_assert(Smem::total + 1024 <= 232448, "decode kernel shared memory exceeds the 227 KB per-CTA limit");
@@ -113,7 +109,6 @@ struct Unit {
   int r, c, h, n_chunks, kv_len, kv_begin, kv_end_tc, n_tiles;
   int last_chunk;
 };
-static_assert(sizeof(Unit) <= 40, "Unit must fit its smem slot");
 
 // Work unit `pos` of the size-sorted order (metadata.cu): the hkv heads of an item are adjacent positions
 // (neighbouring CTAs stream the same token rows).
@@ -132,7 +127,7 @@ __device__ __forceinline__ Unit get_unit(int pos, int hkv, int chunk_tokens, con
   u.last_chunk = (u.c == u.n_chunks - 1);
   u.kv_end_tc = u.last_chunk ? kv_end - 1 : kv_end;  // the appended token is handled on CUDA cores
   const int n = u.kv_end_tc - u.kv_begin;
-  u.n_tiles = n > 0 ? (n + kTileN - 1) / kTileN : 0;
+  u.n_tiles = n > 0 ? (n + kKvTileRows - 1) / kKvTileRows : 0;
   return u;
 }
 
@@ -151,7 +146,6 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   const int tid = threadIdx.x, warp = tid / kWarp, lane = tid % kWarp;
   auto bar = [&](int i) { return sbase + Smem::bars + i * 8; };
   float* red = reinterpret_cast<float*>(smem + Smem::red);
-  uint8_t* sUnits = smem + Smem::units;
 
   // ---------------------------------------------------------------- setup that touches no global memory
   // zero the Q operand buffers whose padding rows (heads >= G) are never written again
@@ -196,32 +190,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   if (!p.early) pdl_wait();
   pdl_launch_dependents();
   const int chunk_tokens = p.plan[0];
-  const int total_units = p.plan[1] * p.hkv;
   const int32_t* order = p.plan + kPlanHeader + p.bs + 1;
-  const int32_t* seq_lens = p.seq_lens;
-  // This CTA's k-th unit is position k*grid + (k even ? cta : grid-1-cta) of the size-sorted order
-  // ("snake" dealing): per-CTA work is balanced to within about one tile.
-  const int grid = gridDim.x, cta = blockIdx.x;
-  const int n_rounds = (total_units + grid - 1) / grid;
-  auto pos_of = [&](int k) { return k * grid + ((k & 1) ? grid - 1 - cta : cta); };
+  const auto units = deal_units<Unit, kUnitSlotBytes, kMaxUnitsSmem>(
+      smem + Smem::units, p.plan[1] * p.hkv,
+      [&](int pos) { return get_unit(pos, p.hkv, chunk_tokens, order, p.seq_lens); });
 
   // ---------------------------------------------------------------- one-time setup
-  // every role walks the same unit list: decode it once, in parallel, into smem
-  for (int k = tid; k < kMaxUnitsSmem && k < n_rounds; k += kThreads) {
-    const int pos = pos_of(k);
-    Unit u;
-    u.n_tiles = -1;  // marks "no unit in this round"
-    if (pos < total_units) u = get_unit(pos, p.hkv, chunk_tokens, order, seq_lens);
-    *reinterpret_cast<Unit*>(sUnits + k * 40) = u;
-  }
-  auto unit_at = [&](int k) {
-    if (k < kMaxUnitsSmem) return *reinterpret_cast<const Unit*>(sUnits + k * 40);
-    const int pos = pos_of(k);
-    Unit u;
-    u.n_tiles = -1;
-    if (pos < total_units) u = get_unit(pos, p.hkv, chunk_tokens, order, seq_lens);
-    return u;
-  };
+  units.stage(tid, kThreads);
   fence_proxy_async_smem();  // zero-fill above must be visible to wgmma operand reads
   __syncthreads();
   if (warp < 4) {
@@ -238,55 +213,34 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       const CUtensorMap* bmap = kind == 0 ? &box_k : &box_v;
       const int full0 = kind == 0 ? kFullK : kFullV, empty0 = kind == 0 ? kEmptyK : kEmptyV;
       const uint32_t ring = sbase + (kind == 0 ? Smem::kring : Smem::vring);
-      uint32_t tile_count = 0;
-      for (int k = 0; k < n_rounds; ++k) {
-        const Unit u = unit_at(k);
+      RingCursor<kStages> kv;
+      for (int k = 0; k < units.n_rounds; ++k) {
+        const Unit u = units.at(k);
         if (u.n_tiles <= 0) continue;
         const int32_t* slots = p.slot_table + (int64_t)u.r * p.st_stride;
         const int col0 = u.h * kD;
-        // four slots of row group `grp` (rows 4*grp..4*grp+3 of tile t); invalid rows -> out of range
-        auto load_group = [&](int t, int grp) {
-          int4 rr;
-          const int pos0 = u.kv_begin + t * kTileN + grp * 4;
-          if (pos0 + 3 < u.kv_end_tc) {
-            rr = __ldg(reinterpret_cast<const int4*>(slots + pos0));
-          } else {
-            rr.x = pos0 + 0 < u.kv_end_tc ? __ldg(slots + pos0 + 0) : p.num_slots;
-            rr.y = pos0 + 1 < u.kv_end_tc ? __ldg(slots + pos0 + 1) : p.num_slots;
-            rr.z = pos0 + 2 < u.kv_end_tc ? __ldg(slots + pos0 + 2) : p.num_slots;
-            rr.w = pos0 + 3 < u.kv_end_tc ? __ldg(slots + pos0 + 3) : p.num_slots;
-          }
-          return rr;
-        };
         if (rb == 0) {
-          // ---- row mode: this warp owns 64 rows; lane = (row group of four, half)
-          const int grp = (warp & 1) * 16 + (lane >> 1), half = lane & 1;
-          int4 nxt = make_int4(0, 0, 0, 0);
-          if (u.n_tiles > 0) nxt = load_group(0, grp);
-          for (int t = 0; t < u.n_tiles; ++t, ++tile_count) {
+          // ---- row mode: this warp owns 64 rows
+          const KvLane L = KvLane::group(lane, warp & 1);
+          auto load_group = [&](int t) {
+            return kv_slot_group(slots, u.kv_begin + t * kKvTileRows + L.row, u.kv_end_tc, p.num_slots);
+          };
+          int4 nxt = load_group(0);
+          for (int t = 0; t < u.n_tiles; ++t, kv.advance()) {
             const int4 cur = nxt;
-            if (t + 1 < u.n_tiles) nxt = load_group(t + 1, grp);
-            const uint32_t stage = tile_count % kStages, phase = (tile_count / kStages) & 1;
-            mbar_wait(bar(empty0 + stage), phase ^ 1);
-            if ((warp & 1) == 0 && lane == 0) mbar_arrive_expect_tx(bar(full0 + stage), kStageBytes);
+            if (t + 1 < u.n_tiles) nxt = load_group(t + 1);
+            kv.wait_empty(bar(empty0));
+            if ((warp & 1) == 0 && lane == 0) mbar_arrive_expect_tx(bar(full0 + kv.stage()), kKvTileBytes);
             __syncwarp();
-            const uint32_t dst = ring + stage * kStageBytes + half * kHalfBytes + grp * 512;
-            const uint32_t fb = bar(full0 + stage);
-            const int col = col0 + half * 64;
-            tma_load_2d(dst, gmap, fb, col, cur.x);
-            tma_load_2d(dst + 128, gmap, fb, col, cur.y);
-            tma_load_2d(dst + 256, gmap, fb, col, cur.z);
-            tma_load_2d(dst + 384, gmap, fb, col, cur.w);
+            tma_load_group(L.dst(ring, kv.stage()), gmap, bar(full0 + kv.stage()), L.col(col0), cur);
           }
         } else {
-          // ---- box mode: lane = (box, half); a box is rb consecutive positions of one page
-          const int n_instr = (kTileN / rb) * 2;  // <= 32
+          // ---- box mode
+          const KvLane L = KvLane::box(lane, rb);
+          const int n_instr = KvLane::box_lanes(rb);  // <= 32
           const CUtensorMap* tmap = kind == 0 ? &tail_k : &tail_v;
-          for (int t = 0; t < u.n_tiles; ++t, ++tile_count) {
-            const uint32_t stage = tile_count % kStages, phase = (tile_count / kStages) & 1;
-            const int tile_begin = u.kv_begin + t * kTileN;
-            const int box = lane >> 1, half = lane & 1;
-            const int pb = tile_begin + box * rb;
+          for (int t = 0; t < u.n_tiles; ++t, kv.advance()) {
+            const int pb = u.kv_begin + t * kKvTileRows + L.row;
             // Rows this lane loads.  Exact tail: a box wholly inside the range is one rb-row box, the box
             // holding the end of the range is cut to its valid rows rounded up to 8-row boxes, and a box
             // wholly past the end is not issued.  Otherwise every box is loaded whole: one reaching past
@@ -301,13 +255,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             if (lane < n_instr && left > 0) first_slot = __ldg(slots + pb);
             // the stage's transaction bytes are exactly the rows the lanes issue below
             const uint32_t tx_bytes = __reduce_add_sync(0xffffffffu, (uint32_t)rows) * 128u;
-            mbar_wait(bar(empty0 + stage), phase ^ 1);
-            if (lane == 0) mbar_arrive_expect_tx(bar(full0 + stage), tx_bytes);
+            kv.wait_empty(bar(empty0));
+            const uint32_t fb = bar(full0 + kv.stage());
+            if (lane == 0) mbar_arrive_expect_tx(fb, tx_bytes);
             __syncwarp();
             if (rows > 0) {
-              const uint32_t dst = ring + stage * kStageBytes + half * kHalfBytes + box * rb * 128;
-              const uint32_t fb = bar(full0 + stage);
-              const int col = col0 + half * 64;
+              const uint32_t dst = L.dst(ring, kv.stage());
+              const int col = L.col(col0);
               if (rows == rb) {
                 tma_load_2d(dst, bmap, fb, col, first_slot);
               } else {
@@ -322,16 +276,17 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   } else if (warp == kWarpQ) {
     // ============================================================ Q loader
     if (p.early) pdl_wait();
-    uint32_t unit_count = 0, epi_count = 0;
-    for (int k = 0; k < n_rounds; ++k) {
-      const Unit u = unit_at(k);
-      if (u.n_tiles < 0) continue;
+    RingCursor<2> qr;
+    RingCursor<kEpiSlots> er;
+    for (int k = 0; k < units.n_rounds; ++k) {
+      const Unit u = units.at(k);
+      if (units.none(u)) continue;
       const bool need_q = u.n_tiles > 0;                 // the tensor core needs the Q operand
       const bool need_epi = p.fuse && u.last_chunk;      // the epilogue needs roped q / k rows
       if (!need_q && !need_epi) continue;
-      const uint32_t qb = unit_count & 1, es = epi_count % kEpiSlots;
-      if (need_q) mbar_wait(bar(kQEmpty + qb), ((unit_count >> 1) & 1) ^ 1);
-      if (need_epi) mbar_wait(bar(kEpiEmpty + es), ((epi_count / kEpiSlots) & 1) ^ 1);
+      const uint32_t qb = qr.stage(), es = er.stage();
+      if (need_q) qr.wait_empty(bar(kQEmpty));
+      if (need_epi) er.wait_empty(bar(kEpiEmpty));
       uint8_t* qdst = smem + Smem::qbuf + qb * kQBufBytes;
       if (!p.fuse) {
         for (int idx = lane; idx < G * 16; idx += kWarp) {
@@ -367,8 +322,8 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
         if (need_q) mbar_arrive(bar(kQFull + qb));
         if (need_epi) mbar_arrive(bar(kEpiFull + es));
       }
-      if (need_q) ++unit_count;
-      if (need_epi) ++epi_count;
+      if (need_q) qr.advance();
+      if (need_epi) er.advance();
     }
   } else if (warp >= 4 && warp < 8) {
     // ============================================================ consumer warpgroup (128 threads)
@@ -384,10 +339,14 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     float* red_max = red;          // [4 warps][8 heads]
     float* red_sum0 = red + 32;    // [2 parity][4][8]
     float* red_new0 = red + 96;    // [2 parity][4][8]
-    uint32_t tile_count = 0, q_count = 0, fin_count = 0, epi_fin = 0, unit_par = 0;
-    for (int k = 0; k < n_rounds; ++k) {
-      const Unit u = unit_at(k);
-      if (u.n_tiles < 0) continue;  // no unit for this CTA in the last round
+    RingCursor<kStages> kv;
+    RingCursor<2> qr;
+    RingCursor<kFinRing> fr;
+    RingCursor<kEpiSlots> er;
+    uint32_t unit_par = 0;
+    for (int k = 0; k < units.n_rounds; ++k) {
+      const Unit u = units.at(k);
+      if (units.none(u)) continue;
       float acc[2][4], l_thr[2], m_run[2];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
@@ -428,14 +387,14 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
         }
       }
       if (u.n_tiles > 0) {
-        const uint32_t qb = q_count & 1;
-        mbar_wait(bar(kQFull + qb), (q_count >> 1) & 1);
+        const uint32_t qb = qr.stage();
+        qr.wait_full(bar(kQFull));
         const uint32_t qa = sbase + Smem::qbuf + qb * kQBufBytes;
-        for (int j = 0; j < u.n_tiles; ++j, ++tile_count) {
-          const uint32_t stage = tile_count % kStages, sphase = (tile_count / kStages) & 1;
+        for (int j = 0; j < u.n_tiles; ++j, kv.advance()) {
+          const uint32_t stage = kv.stage();
           // ---- S^T = K_tile . Q^T: A = K rows (K-major, 128B swizzle), B = Q rows (K-major)
-          mbar_wait(bar(kFullK + stage), sphase);
-          const uint32_t kb = sbase + Smem::kring + stage * kStageBytes;
+          kv.wait_full(bar(kFullK));
+          const uint32_t kb = sbase + Smem::kring + stage * kKvTileBytes;
           float s[2][4];
 #pragma unroll
           for (int mb = 0; mb < 2; ++mb)
@@ -446,7 +405,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
             for (int kk = 0; kk < 8; ++kk) {
-              const uint64_t da = make_smem_desc(kb + mb * 8192 + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
+              const uint64_t da = make_smem_desc(kb + mb * 8192 + (kk >> 2) * kKvHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
               const uint64_t db = make_smem_desc(qa + (kk >> 2) * 1024 + (kk & 3) * 32, 16, 1024, kLayoutSW128);
               wgmma_m64n8k16_ss<0>(s[mb], da, db, kk > 0, tsel);
             }
@@ -457,16 +416,16 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             mbar_arrive(bar(kEmptyK + stage));                      // the K tile is dead
             if (j + 1 == u.n_tiles) mbar_arrive(bar(kQEmpty + qb));  // last QK of the unit
           }
-          const int n_valid = u.kv_end_tc - (u.kv_begin + j * kTileN);  // >= 1
-          if (p.box_rows > 0 && n_valid < kTileN) {
+          const int n_valid = u.kv_end_tc - (u.kv_begin + j * kKvTileRows);  // >= 1
+          if (p.box_rows > 0 && n_valid < kKvTileRows) {
             // box mode, last tile of the range: the V rows past the end hold the rest of the page or
             // an earlier tile of this stage (possibly NaN bit patterns): zero them so that 0 * garbage
             // cannot reach the output
-            mbar_wait(bar(kFullV + stage), sphase);
-            uint8_t* vt = smem + Smem::vring + stage * kStageBytes;
-            for (int idx = ct; idx < (kTileN - n_valid) * 16; idx += 128) {
+            kv.wait_full(bar(kFullV));
+            uint8_t* vt = smem + Smem::vring + stage * kKvTileBytes;
+            for (int idx = ct; idx < (kKvTileRows - n_valid) * 16; idx += 128) {
               const int row = n_valid + (idx >> 4), c16 = idx & 15;
-              *reinterpret_cast<uint4*>(vt + (c16 >> 3) * kHalfBytes + row * 128 + (c16 & 7) * 16) = make_uint4(0, 0, 0, 0);
+              *reinterpret_cast<uint4*>(vt + (c16 >> 3) * kKvHalfBytes + row * 128 + (c16 & 7) * 16) = make_uint4(0, 0, 0, 0);
             }
             fence_proxy_async_smem();
           }
@@ -517,8 +476,8 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           fence_proxy_async_smem();  // P^T (and zeroed V rows) visible to the tensor core
           named_bar_sync(1, 128);    // every warp's P^T is written; the tile maxima may be overwritten
           // ---- O^T += V_tile^T . P^T: A = V rows read MN-major, B = P^T (K-major, no swizzle)
-          mbar_wait(bar(kFullV + stage), sphase);
-          const uint32_t vb = sbase + Smem::vring + stage * kStageBytes;
+          kv.wait_full(bar(kFullV));
+          const uint32_t vb = sbase + Smem::vring + stage * kKvTileBytes;
           const uint32_t pb = sbase + Smem::pbuf;
           wgmma_fence();
 #pragma unroll
@@ -526,7 +485,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
 #pragma unroll
             for (int kk = 0; kk < 8; ++kk) {
               // 16 keys = two 8-key swizzle atoms of 1024 B; dims 64..127 in the second half (+16 KB)
-              const uint64_t da = make_smem_desc(vb + mb * kHalfBytes + kk * 2048, kHalfBytes, 1024, kLayoutSW128);
+              const uint64_t da = make_smem_desc(vb + mb * kKvHalfBytes + kk * 2048, kKvHalfBytes, 1024, kLayoutSW128);
               const uint64_t db = make_smem_desc(pb + kk * 256, 128, 1024, kLayoutNone);
               wgmma_m64n8k16_ss<kTransV ? 1 : 0>(acc[mb], da, db, 1u, tsel);
             }
@@ -535,7 +494,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           __syncwarp();
           if (lane == 0) mbar_arrive(bar(kEmptyV + stage));
         }
-        ++q_count;
+        qr.advance();
       }
 
       // ---- unit epilogue on CUDA cores: row sums, the appended token (score, value, pool append), output.
@@ -545,11 +504,11 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       float* red_new = red_new0 + unit_par * 32;
       unit_par ^= 1;
       const bool epi = p.fuse && u.last_chunk;
-      const uint32_t es = epi_fin % kEpiSlots;
+      const uint32_t es = er.stage();
       if (epi) {
         // fused mode: the Q loader left the roped q rows of the group and the roped new k row in the ring
-        mbar_wait(bar(kEpiFull + es), (epi_fin / kEpiSlots) & 1);
-        ++epi_fin;
+        er.wait_full(bar(kEpiFull));
+        er.advance();
         const uint8_t* esrc = smem + Smem::epi + es * kEpiSlotBytes;
 #pragma unroll
         for (int x = 0; x < 4; ++x) {
@@ -635,10 +594,9 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
         // only pay an mbarrier arrive; the release/acquire pair orders the partial stores above
         // before the combiner's device-scope fence + arrival counter.
         if (p.fused_combine) {
-          const uint32_t slot = fin_count % kFinRing;
-          mbar_wait(bar(kFinEmpty + slot), ((fin_count / kFinRing) & 1) ^ 1);
-          mbar_arrive(bar(kFinFull + slot));
-          ++fin_count;
+          fr.wait_empty(bar(kFinEmpty));
+          mbar_arrive(bar(kFinFull + fr.stage()));
+          fr.advance();
         }
       }
     }
@@ -648,13 +606,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     // whoever arrives last merges all partials (flash-decoding reduction) and writes the output.
     if (p.early) pdl_wait();
     if (p.fused_combine) {
-      uint32_t fin_count = 0;
-      for (int k = 0; k < n_rounds; ++k) {
-        const Unit u = unit_at(k);
-        if (u.n_tiles < 0 || u.n_chunks == 1) continue;
-        const uint32_t slot = fin_count % kFinRing;
-        mbar_wait(bar(kFinFull + slot), (fin_count / kFinRing) & 1);
-        ++fin_count;
+      RingCursor<kFinRing> fr;
+      for (int k = 0; k < units.n_rounds; ++k) {
+        const Unit u = units.at(k);
+        if (units.none(u) || u.n_chunks == 1) continue;
+        const uint32_t slot = fr.stage();
+        fr.wait_full(bar(kFinFull));
+        fr.advance();
         __threadfence();
         int last = 0;
         if (lane == 0) {

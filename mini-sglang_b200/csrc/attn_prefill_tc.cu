@@ -19,7 +19,6 @@
 //               max / sum need two shuffles; K/V tiles that are fully masked for all 64 rows are skipped.
 // The producer warpgroup hands registers to the consumers (setmaxnreg): 128 x 40 + 256 x 232 = 384 x 168.
 #include "attn.cuh"
-#include "sm90.cuh"
 
 #include <type_traits>
 
@@ -30,20 +29,17 @@ using namespace sm90;
 
 constexpr int kD = kHeadDim;
 constexpr int kBM = 128;                   // query rows per unit (two consumer warpgroups x 64)
-constexpr int kBN = 128;                   // keys per tile
 constexpr int kStages = 2;                 // K ring depth = V ring depth
 constexpr int kThreads = 384;
-constexpr int kHalfBytes = 128 * 128;      // [128 rows x 64 cols] 16-bit, 128B-swizzled: 16 KB
-constexpr int kTileBytes = 2 * kHalfBytes; // 32 KB
-constexpr int kMaxUnitsSmem = 64;
+constexpr int kUnitSlotBytes = 48, kMaxUnitsSmem = 64;
 
 struct Smem {
   static constexpr int q = 0;                                // one 128-row Q tile: 32 KB
-  static constexpr int kring = kTileBytes;                   // kStages x 32 KB
-  static constexpr int vring = kring + kStages * kTileBytes;
-  static constexpr int bars = vring + kStages * kTileBytes;  // 10 mbarriers
+  static constexpr int kring = kKvTileBytes;                   // one 32 KB tile per stage
+  static constexpr int vring = kring + kStages * kKvTileBytes;
+  static constexpr int bars = vring + kStages * kKvTileBytes;  // 10 mbarriers
   static constexpr int units = bars + 16 * 8;
-  static constexpr int total = units + kMaxUnitsSmem * 48;
+  static constexpr int total = units + kMaxUnitsSmem * kUnitSlotBytes;
 };
 static_assert(Smem::total + 1024 <= 232448, "prefill kernel shared memory exceeds the 227 KB per-CTA limit");
 enum Bar { kFullK = 0, kEmptyK = 2, kFullV = 4, kEmptyV = 6, kQFull = 8, kQEmpty = 9 };
@@ -74,7 +70,6 @@ struct Params {
 struct Unit {
   int r, q_start, q_len, q_begin, kv_len, cached, kv_hi, n_tiles, h, head, owner;
 };
-static_assert(sizeof(Unit) <= 48, "Unit must fit its smem slot");
 
 __device__ __forceinline__ Unit get_unit(int pos, int hq, int group, const int32_t* items,
                                          const int32_t* seq_lens, const int32_t* cu_q) {
@@ -91,7 +86,7 @@ __device__ __forceinline__ Unit get_unit(int pos, int hq, int group, const int32
   u.kv_len = seq_lens[u.r];
   u.cached = u.kv_len - u.q_len;
   u.kv_hi = min(u.kv_len, u.cached + min(u.q_len, u.q_start + kBM));
-  u.n_tiles = (u.kv_hi + kBN - 1) / kBN;
+  u.n_tiles = (u.kv_hi + kKvTileRows - 1) / kKvTileRows;
   return u;
 }
 
@@ -117,31 +112,15 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid / kWarp, lane = tid % kWarp;
   auto bar = [&](int i) { return sbase + Smem::bars + i * 8; };
-  uint8_t* sUnits = smem + Smem::units;
 
   const int group = p.hq / p.hkv;
-  const int total_units = p.plan[0] * p.hq;
   const int32_t* items = p.plan + 4;
-  const int grid = gridDim.x, cta = blockIdx.x;
-  const int n_rounds = (total_units + grid - 1) / grid;
-  auto pos_of = [&](int k) { return k * grid + ((k & 1) ? grid - 1 - cta : cta); };
+  const auto units = deal_units<Unit, kUnitSlotBytes, kMaxUnitsSmem>(
+      smem + Smem::units, p.plan[0] * p.hq,
+      [&](int pos) { return get_unit(pos, p.hq, group, items, p.seq_lens, p.cu_q); });
 
   // ---------------------------------------------------------------- one-time setup
-  for (int k = tid; k < kMaxUnitsSmem && k < n_rounds; k += kThreads) {
-    const int pos = pos_of(k);
-    Unit u;
-    u.n_tiles = -1;
-    if (pos < total_units) u = get_unit(pos, p.hq, group, items, p.seq_lens, p.cu_q);
-    *reinterpret_cast<Unit*>(sUnits + k * 48) = u;
-  }
-  auto unit_at = [&](int k) {
-    if (k < kMaxUnitsSmem) return *reinterpret_cast<const Unit*>(sUnits + k * 48);
-    const int pos = pos_of(k);
-    Unit u;
-    u.n_tiles = -1;
-    if (pos < total_units) u = get_unit(pos, p.hq, group, items, p.seq_lens, p.cu_q);
-    return u;
-  };
+  units.stage(tid, kThreads);
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(bar(kFullK + s), 1);
@@ -177,14 +156,15 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     const CUtensorMap* bmap = kind == 0 ? &box_k : &box_v;
     const int full0 = kind == 0 ? kFullK : kFullV, empty0 = kind == 0 ? kEmptyK : kEmptyV;
     const uint32_t ring = sbase + (kind == 0 ? Smem::kring : Smem::vring);
-    uint32_t tile_count = 0, unit_count = 0;
+    RingCursor<kStages> kv;
+    RingCursor<1> qr;
     // ---- fused KV append: the tile of a unit that holds the unit's own new tokens is written to the
     // pool straight from shared memory (TMA store) when its ring slot is recycled -- no extra loads,
     // no extra launch.  Ownership: positions [cached + q_start, cached + min(q_len, q_start + 128)) of
     // kv head h belong to the unit of query tile q_start and the first query head of the group.
     struct Pending {
       int valid, lo, hi, tile_begin, col0;
-      uint32_t phase;
+      RingCursor<kStages> at;  // ring position of the tile; its stage is the entry's index
       const int32_t* slots;
     } pend[kStages];
     for (int s = 0; s < kStages; ++s) pend[s].valid = 0;
@@ -193,31 +173,28 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     // valid: 0 = nothing, 1 = tile issued (append once it has landed), 2 = stores issued
     auto issue_stores = [&](int stage) {  // whole warp; the tile has landed
       Pending& pd = pend[stage];
-      const uint32_t base = ring + stage * kTileBytes;
       if (rb > 0) {
-        const int n_instr = (kBN / rb) * 2;
-        if (lane < n_instr) {
-          const int box = lane >> 1, half = lane & 1;
-          const int pb = pd.tile_begin + box * rb;
-          const uint32_t src = base + half * kHalfBytes + box * rb * 128;
-          const int col = pd.col0 + half * 64;
+        if (lane < KvLane::box_lanes(rb)) {
+          const KvLane L = KvLane::box(lane, rb);
+          const int pb = pd.tile_begin + L.row;
+          const uint32_t src = L.dst(ring, stage);
           if (pb >= pd.lo && pb + rb <= pd.hi) {
-            tma_store_2d(smap_box, src, col, __ldg(pd.slots + pb));
+            tma_store_2d(smap_box, src, L.col(pd.col0), __ldg(pd.slots + pb));
           } else {
             for (int i = 0; i < rb; ++i)
-              if (pb + i >= pd.lo && pb + i < pd.hi) tma_store_2d(smap_row, src + i * 128, col, __ldg(pd.slots + pb + i));
+              if (pb + i >= pd.lo && pb + i < pd.hi)
+                tma_store_2d(smap_row, src + i * 128, L.col(pd.col0), __ldg(pd.slots + pb + i));
           }
         }
       } else {
 #pragma unroll
         for (int it = 0; it < 2; ++it) {
-          const int grp = (lane >> 1) + it * 16, half = lane & 1;
-          const int pos0 = pd.tile_begin + grp * 4;
+          const KvLane L = KvLane::group(lane, it);
+          const int pos0 = pd.tile_begin + L.row;
 #pragma unroll
           for (int i = 0; i < 4; ++i)
             if (pos0 + i >= pd.lo && pos0 + i < pd.hi)
-              tma_store_2d(smap_row, base + half * kHalfBytes + (grp * 4 + i) * 128, pd.col0 + half * 64,
-                           __ldg(pd.slots + pos0 + i));
+              tma_store_2d(smap_row, L.dst(ring, stage) + i * 128, L.col(pd.col0), __ldg(pd.slots + pos0 + i));
         }
       }
       bulk_commit();
@@ -226,7 +203,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     };
     // opportunistic: append a tile as soon as it has landed (the tensor core may still be reading it)
     auto try_store = [&](int stage) {
-      if (pend[stage].valid == 1 && mbar_test_wait(bar(full0 + stage), pend[stage].phase)) issue_stores(stage);
+      if (pend[stage].valid == 1 && mbar_test_wait(bar(full0 + stage), pend[stage].at.phase())) issue_stores(stage);
     };
     // before a ring slot is overwritten: its tile has landed and been consumed
     auto flush_stage = [&](int stage) {
@@ -236,8 +213,8 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
         pend[stage].valid = 0;
       }
     };
-    for (int k = 0; k < n_rounds; ++k) {
-      const Unit u = unit_at(k);
+    for (int k = 0; k < units.n_rounds; ++k) {
+      const Unit u = units.at(k);
       if (u.n_tiles <= 0) continue;
       const int32_t* slots = p.slot_table + (int64_t)u.r * p.st_stride;
       const int col0 = u.h * kD;
@@ -249,11 +226,11 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
       auto load_q = [&]() {
         // rows past the tensor end are zero filled, rows past the request's end belong to the next
         // request: computed, never stored
-        mbar_wait(bar(kQEmpty), (unit_count & 1) ^ 1);
+        qr.wait_empty(bar(kQEmpty));
         if (lane == 0) {
-          mbar_arrive_expect_tx(bar(kQFull), (uint32_t)kTileBytes);
+          mbar_arrive_expect_tx(bar(kQFull), (uint32_t)kKvTileBytes);
           for (int half = 0; half < 2; ++half)
-            tma_load_2d(sbase + Smem::q + half * kHalfBytes, &map_q, bar(kQFull), u.head * kD + half * 64,
+            tma_load_2d(sbase + Smem::q + half * kKvHalfBytes, &map_q, bar(kQFull), u.head * kD + half * 64,
                         u.q_begin + u.q_start);
         }
         __syncwarp();
@@ -272,50 +249,42 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
           else tma_load_2d(dst + i * 128, nmap, fb, col, u.q_begin + pos - u.cached);
         }
       };
-      for (int t = 0; t < u.n_tiles; ++t, ++tile_count) {
-        const uint32_t stage = tile_count % kStages, phase = (tile_count / kStages) & 1;
-        const int tile_begin = t * kBN;
+      for (int t = 0; t < u.n_tiles; ++t, kv.advance()) {
+        const uint32_t stage = kv.stage();
+        const uint32_t fb = bar(full0 + stage);
+        const int tile_begin = t * kKvTileRows;
         if (rb > 0) {
-          const int n_instr = (kBN / rb) * 2;
-          const int box = lane >> 1, half = lane & 1;
-          const int pb = tile_begin + box * rb;
+          const int n_instr = KvLane::box_lanes(rb);
+          const KvLane L = KvLane::box(lane, rb);
+          const int pb = tile_begin + L.row;
           const bool old_box = pb + rb <= u.cached, new_box = pb >= u.cached;
           int first_slot = p.num_slots;
           if (lane < n_instr && old_box) first_slot = __ldg(slots + pb);
-          mbar_wait(bar(empty0 + stage), phase ^ 1);
+          kv.wait_empty(bar(empty0));
           flush_stage(stage);
-          if (lane == 0) mbar_arrive_expect_tx(bar(full0 + stage), kTileBytes);
+          if (lane == 0) mbar_arrive_expect_tx(fb, kKvTileBytes);
           __syncwarp();
           if (lane < n_instr) {
-            const uint32_t dst = ring + stage * kTileBytes + half * kHalfBytes + box * rb * 128;
-            const uint32_t fb = bar(full0 + stage);
-            const int col = col0 + half * 64;
+            const uint32_t dst = L.dst(ring, stage);
+            const int col = L.col(col0);
             if (old_box) tma_load_2d(dst, bmap, fb, col, first_slot);
             else if (new_box) tma_load_2d(dst, nbmap, fb, col, u.q_begin + pb - u.cached);
             else load_rows_one_by_one(dst, fb, col, pb, rb);  // the box straddling cached_len
           }
         } else {
           // row mode: 32 row groups of four x 2 halves = 2 groups per lane, one single-row box per row
-          mbar_wait(bar(empty0 + stage), phase ^ 1);
+          kv.wait_empty(bar(empty0));
           flush_stage(stage);
-          if (lane == 0) mbar_arrive_expect_tx(bar(full0 + stage), kTileBytes);
+          if (lane == 0) mbar_arrive_expect_tx(fb, kKvTileBytes);
           __syncwarp();
 #pragma unroll
           for (int it = 0; it < 2; ++it) {
-            const int grp = (lane >> 1) + it * 16, half = lane & 1;
-            const int pos0 = tile_begin + grp * 4;
-            const uint32_t dst = ring + stage * kTileBytes + half * kHalfBytes + grp * 512;
-            const uint32_t fb = bar(full0 + stage);
-            const int col = col0 + half * 64;
-            if (pos0 + 4 <= u.cached) {
-              const int4 rr = __ldg(reinterpret_cast<const int4*>(slots + pos0));
-              tma_load_2d(dst, gmap, fb, col, rr.x);
-              tma_load_2d(dst + 128, gmap, fb, col, rr.y);
-              tma_load_2d(dst + 256, gmap, fb, col, rr.z);
-              tma_load_2d(dst + 384, gmap, fb, col, rr.w);
-            } else {
-              load_rows_one_by_one(dst, fb, col, pos0, 4);
-            }
+            const KvLane L = KvLane::group(lane, it);
+            const int pos0 = tile_begin + L.row;
+            if (pos0 + 4 <= u.cached)
+              tma_load_group(L.dst(ring, stage), gmap, fb, L.col(col0), kv_slot_group(slots, pos0, u.cached, p.num_slots));
+            else
+              load_rows_one_by_one(L.dst(ring, stage), fb, L.col(col0), pos0, 4);
           }
         }
         if (kind == 0 && t == 0) load_q();
@@ -323,23 +292,23 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
         for (int s2 = 0; s2 < kStages; ++s2)
           if (s2 != (int)stage) try_store(s2);
         // does this tile hold rows this unit has to append?
-        const int lo = max(own_lo, tile_begin), hi = min(own_hi, tile_begin + kBN);
+        const int lo = max(own_lo, tile_begin), hi = min(own_hi, tile_begin + kKvTileRows);
         if (owner && lo < hi) {
           pend[stage].valid = 1;
           pend[stage].lo = lo;
           pend[stage].hi = hi;
           pend[stage].tile_begin = tile_begin;
           pend[stage].col0 = col0;
-          pend[stage].phase = phase;
+          pend[stage].at = kv;
           pend[stage].slots = slots;
         }
       }
-      ++unit_count;
+      qr.advance();
     }
     // tiles still waiting for their append: wait until they have landed, store, drain
     for (int s = 0; s < kStages; ++s)
       if (pend[s].valid == 1) {
-        mbar_wait(bar(full0 + s), pend[s].phase);
+        mbar_wait(bar(full0 + s), pend[s].at.phase());
         issue_stores(s);
       }
     bulk_wait0();
@@ -354,9 +323,10 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     // columns 8i + 2*(lane%4) (+1), i = 0..15
     const int ra = wg * 64 + 16 * cw + (lane >> 2);
     const int cq = 2 * (lane & 3);
-    uint32_t tile_count = 0, unit_count = 0;
-    for (int k = 0; k < n_rounds; ++k) {
-      const Unit u = unit_at(k);
+    RingCursor<kStages> kv;
+    RingCursor<1> qr;
+    for (int k = 0; k < units.n_rounds; ++k) {
+      const Unit u = units.at(k);
       if (u.n_tiles <= 0) continue;
       // keys [0, vis_end) are visible to a query row; the warpgroup's last row bounds the tiles it needs
       const int vis0 = min(u.cached + u.q_start + ra + 1, u.kv_len);
@@ -366,24 +336,24 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
 #pragma unroll
       for (int i = 0; i < 64; ++i) o[i] = 0.f;
       float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-      mbar_wait(bar(kQFull), unit_count & 1);
-      ++unit_count;
+      qr.wait_full(bar(kQFull));
+      qr.advance();
       const uint32_t qa = sbase + Smem::q + wg * 8192;  // 64 rows x 128 B into each half
-      for (int j = 0; j < u.n_tiles; ++j, ++tile_count) {
-        const uint32_t stage = tile_count % kStages, phase = (tile_count / kStages) & 1;
-        const int tile_begin = j * kBN;
+      for (int j = 0; j < u.n_tiles; ++j, kv.advance()) {
+        const uint32_t stage = kv.stage();
+        const int tile_begin = j * kKvTileRows;
         const bool active = tile_begin < wg_vis;  // warpgroup-uniform
-        mbar_wait(bar(kFullK + stage), phase);
+        kv.wait_full(bar(kFullK));
         float s[64];
         if (active) {
-          const uint32_t kb = sbase + Smem::kring + stage * kTileBytes;
+          const uint32_t kb = sbase + Smem::kring + stage * kKvTileBytes;
 #pragma unroll
           for (int i = 0; i < 64; ++i) s[i] = 0.f;
           wgmma_fence();
 #pragma unroll
           for (int kk = 0; kk < 8; ++kk) {
-            const uint64_t da = make_smem_desc(qa + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
-            const uint64_t db = make_smem_desc(kb + (kk >> 2) * kHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
+            const uint64_t da = make_smem_desc(qa + (kk >> 2) * kKvHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
+            const uint64_t db = make_smem_desc(kb + (kk >> 2) * kKvHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
             wgmma_m64n128k16_ss(s, da, db, kk > 0, tsel);
           }
           wgmma_commit();
@@ -436,14 +406,14 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
             pa[kb][3] = pack2<T>(s[8 * kb + 6], s[8 * kb + 7]);
           }
         }
-        mbar_wait(bar(kFullV + stage), phase);
+        kv.wait_full(bar(kFullV));
         if (active) {
-          const uint32_t vb = sbase + Smem::vring + stage * kTileBytes;
+          const uint32_t vb = sbase + Smem::vring + stage * kKvTileBytes;
           wgmma_fence();
 #pragma unroll
           for (int kb = 0; kb < 8; ++kb) {
             // B = V (MN-major): 16 keys = two 8-key swizzle atoms (1024 B each); dims 64..127 at +16 KB
-            const uint64_t db = make_smem_desc(vb + kb * 2048, kHalfBytes, 1024, kLayoutSW128);
+            const uint64_t db = make_smem_desc(vb + kb * 2048, kKvHalfBytes, 1024, kLayoutSW128);
             wgmma_m64n128k16_rs(o, pa[kb], db, 1u, tsel);
           }
           wgmma_commit();

@@ -58,6 +58,18 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// One role's cursor over an S-stage mbarrier ring: use n is stage n % S in phase (n / S) & 1; full0 / empty0 address
+// stage 0 of S consecutive barriers.  "Empty" is awaited in the previous phase, which a fresh barrier has completed.
+template <int S>
+struct RingCursor {
+  uint32_t n = 0;
+  __device__ __forceinline__ uint32_t stage() const { return n % S; }
+  __device__ __forceinline__ uint32_t phase() const { return (n / S) & 1; }
+  __device__ __forceinline__ void wait_full(uint32_t full0) const { mbar_wait(full0 + stage() * 8, phase()); }
+  __device__ __forceinline__ void wait_empty(uint32_t empty0) const { mbar_wait(empty0 + stage() * 8, phase() ^ 1); }
+  __device__ __forceinline__ void advance() { ++n; }
+};
+
 // generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
