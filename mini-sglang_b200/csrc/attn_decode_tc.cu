@@ -14,13 +14,17 @@
 //            * page_size < 8 ("row mode", all four warps): one single-row TMA box per token row and
 //              half; rows past the end of the KV range are out-of-range rows (zero filled), so stale
 //              pool memory is never multiplied in.
-//   warps 4-7 one consumer warpgroup: S^T[128 keys x 8] = K_tile . Q^T and O^T[128 dims x 8] += V_tile^T . P^T
-//            as wgmma m64n8k16 (two 64-row blocks each): the keys / head dims fill M and the <= 8 query
-//            heads of the GQA group sit in N = 8, so no tensor-core row is spent on padding.  Softmax on
-//            the score fragments (tile max across the four warps through smem + a named barrier), P^T to
-//            smem as the 16-bit B operand, O^T stays in registers with the online-softmax rescale.
+//   warps 4-7 one consumer warpgroup: S^T[128 keys x N] = K_tile . Q^T and O^T[128 dims x N] += V_tile^T . P^T
+//            as wgmma m64nNk16 (two 64-row blocks each): the keys / head dims fill M and the query heads of
+//            the GQA group sit in N -- N = 8 for groups of 1-8, N = 16 for groups of 9-16, chosen at compile
+//            time from the group size -- so no tensor-core row is spent on padding.  Softmax on the score
+//            fragments (tile max across the four warps through smem + a named barrier), P^T to smem as the
+//            16-bit B operand, O^T stays in registers with the online-softmax rescale.
 //   warp 8   Q loader: the group's q rows -> swizzled smem operand (double buffered across units).
 //   warp 9   split-KV combiner: the last-arriving chunk of a (request, kv head) merges the partials.
+//
+// Every unit is one (request, chunk, kv head): all G query heads of the group share each K/V tile, so the K/V
+// bytes of a launch do not depend on G.
 //
 // Fused pre-attention (p.fuse, b200_attn_decode_fused): q and the new k row arrive RAW (straight from the
 // qkv projection); the Q loader applies the per-head RMSNorm + neox RoPE of layers/attention.py:50-54 with
@@ -47,26 +51,37 @@ constexpr int kD = kHeadDim;
 constexpr int kStages = 3;
 constexpr int kThreads = 320;
 constexpr int kWarpQ = 8, kWarpCombine = 9;
-constexpr int kNPad = 8;                    // wgmma N (query heads of the group, padded)
-constexpr int kQBufBytes = 2 * 1024;        // two halves of [8 rows x 128 B], 128B-swizzled
-constexpr int kPBufBytes = kNPad * kKvTileRows * 2;  // P^T [8 x 128] 16-bit, no-swizzle K-major
+constexpr int kMaxGroup = 16;               // largest GQA group (query heads per kv head) of the kernel
+template <int G>
+constexpr int kNOf = G <= 8 ? 8 : 16;       // wgmma N: the query heads of the group, padded
 constexpr int kUnitSlotBytes = 40, kMaxUnitsSmem = 96;  // per-CTA work units decoded once into smem
-constexpr int kEpiSlots = 4;                // fused mode: roped (q heads, new k) rows in flight to the epilogue
-constexpr int kEpiSlotBytes = 9 * kD * 2;   // up to 8 q heads + the k row, 128 x 16-bit each
 
+template <int N>
 struct Smem {
+  static_assert(N == 8 || N == 16, "wgmma N of the decode kernel is 8 or 16");
+  static constexpr int kQHalfBytes = N * 128;            // one 64-column half of [N rows x 128 B], 128B-swizzled
+  static constexpr int kQBufBytes = 2 * kQHalfBytes;
+  static constexpr int kPBufBytes = N * kKvTileRows * 2;  // P^T [N x 128] 16-bit, no-swizzle K-major
+  // fused mode: roped (q heads, new k) rows in flight to the epilogue, up to N q heads + the k row of 128 x 16 bit.
+  // N = 16 keeps three slots instead of four: with the doubled Q, P^T and reduction buffers and 17-row slots, four
+  // would need 232704 B with the alignment slack, over the 232448 B a CTA may have.  The ring only lets the Q
+  // loader run ahead of the consumers' epilogues; three slots still cover its two-deep Q ring plus one unit.  The
+  // unit cache keeps its 96 slots, so no batch moves onto the slower decode-from-global path.
+  static constexpr int kEpiSlots = N == 8 ? 4 : 3;
+  static constexpr int kEpiSlotBytes = (N + 1) * kD * 2;
   // offsets from the 1024-aligned base
   static constexpr int kring = 0;                          // K tiles, released right after QK
   static constexpr int vring = kStages * kKvTileBytes;     // V tiles, released after PV
   static constexpr int qbuf = 2 * kStages * kKvTileBytes;
   static constexpr int pbuf = qbuf + 2 * kQBufBytes;
   static constexpr int bars = pbuf + kPBufBytes;           // 32 mbarriers
-  static constexpr int red = bars + 32 * 8;                // floats: tile max [4][8], [2][4][8] row sums, [2][4][8] new-token dots
-  static constexpr int units = red + (32 + 64 + 64) * 4;   // decoded work units
-  static constexpr int epi = units + kMaxUnitsSmem * kUnitSlotBytes;  // fused mode: kEpiSlots x [9][128] 16-bit
+  static constexpr int red = bars + 32 * 8;                // floats: tile max [4][N], [2][4][N] row sums, [2][4][N] new-token dots
+  static constexpr int units = red + 20 * N * 4;           // decoded work units
+  static constexpr int epi = units + kMaxUnitsSmem * kUnitSlotBytes;  // fused mode: kEpiSlots x [N + 1][128] 16-bit
   static constexpr int total = epi + kEpiSlots * kEpiSlotBytes;
 };
-static_assert(Smem::total + 1024 <= 232448, "decode kernel shared memory exceeds the 227 KB per-CTA limit");
+static_assert(Smem<8>::total + 1024 <= 232448, "decode kernel shared memory exceeds the 227 KB per-CTA limit");
+static_assert(Smem<16>::total + 1024 <= 232448, "decode kernel shared memory exceeds the 227 KB per-CTA limit");
 enum Bar { kFullK = 0, kEmptyK = 3, kFullV = 6, kEmptyV = 9, kQFull = 12, kQEmpty = 14, kFinFull = 16, kFinEmpty = 20, kEpiFull = 24, kEpiEmpty = 28 };
 constexpr int kFinRing = 4;  // units in flight between the consumer warps and the combiner warp
 
@@ -131,6 +146,15 @@ __device__ __forceinline__ Unit get_unit(int pos, int hkv, int chunk_tokens, con
   return u;
 }
 
+// wgmma m64nNk16 with both operands in shared memory, N = 8 or 16
+template <int N, int kTransA, typename T>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d, T* tsel) {
+  if constexpr (N == 8)
+    wgmma_m64n8k16_ss<kTransA>(d, da, db, scale_d, tsel);
+  else
+    wgmma_m64n16k16_ss<kTransA>(d, da, db, scale_d, tsel);
+}
+
 template <typename T, int G>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map_k,
@@ -139,6 +163,9 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
                       const __grid_constant__ CUtensorMap box_v,
                       const __grid_constant__ CUtensorMap tail_k,
                       const __grid_constant__ CUtensorMap tail_v) {
+  constexpr int N = kNOf<G>;
+  using Smem = dtc::Smem<N>;
+  constexpr int kE = N / 4;  // accumulator columns (query heads) per thread: h0, h0+1 and, at N = 16, h0+8, h0+9
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B-swizzled tiles
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -149,7 +176,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
 
   // ---------------------------------------------------------------- setup that touches no global memory
   // zero the Q operand buffers whose padding rows (heads >= G) are never written again
-  for (int i = tid; i < (2 * kQBufBytes) / 16; i += kThreads)
+  for (int i = tid; i < (2 * Smem::kQBufBytes) / 16; i += kThreads)
     reinterpret_cast<uint4*>(smem + Smem::qbuf)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
@@ -162,7 +189,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       mbar_init(bar(kFinFull + b), 128);
       mbar_init(bar(kFinEmpty + b), 1);
     }
-    for (int b = 0; b < kEpiSlots; ++b) {
+    for (int b = 0; b < Smem::kEpiSlots; ++b) {
       mbar_init(bar(kEpiFull + b), 1);
       mbar_init(bar(kEpiEmpty + b), 1);
     }
@@ -277,7 +304,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     // ============================================================ Q loader
     if (p.early) pdl_wait();
     RingCursor<2> qr;
-    RingCursor<kEpiSlots> er;
+    RingCursor<Smem::kEpiSlots> er;
     for (int k = 0; k < units.n_rounds; ++k) {
       const Unit u = units.at(k);
       if (units.none(u)) continue;
@@ -287,19 +314,19 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       const uint32_t qb = qr.stage(), es = er.stage();
       if (need_q) qr.wait_empty(bar(kQEmpty));
       if (need_epi) er.wait_empty(bar(kEpiEmpty));
-      uint8_t* qdst = smem + Smem::qbuf + qb * kQBufBytes;
+      uint8_t* qdst = smem + Smem::qbuf + qb * Smem::kQBufBytes;
       if (!p.fuse) {
         for (int idx = lane; idx < G * 16; idx += kWarp) {
           const int g = idx >> 4, cc = idx & 15;
           const Vec8 v = *reinterpret_cast<const Vec8*>(p.q + (int64_t)u.r * p.q_rs +
                                                         (int64_t)(u.h * G + g) * kD + cc * 8);
-          *reinterpret_cast<Vec8*>(qdst + (cc >> 3) * 1024 + sw128_offset(g, cc & 7)) = v;
+          *reinterpret_cast<Vec8*>(qdst + (cc >> 3) * Smem::kQHalfBytes + sw128_offset(g, cc & 7)) = v;
         }
       } else {
         // per-head RMSNorm + RoPE on 16-lane groups, two rows per pass: the G q heads of the group and,
         // for the unit that owns the new token, its k row (row index G).  Uniform trip count: the
         // shuffles inside qknorm_rope_lanes need the whole warp.
-        uint8_t* edst = smem + Smem::epi + es * kEpiSlotBytes;
+        uint8_t* edst = smem + Smem::epi + es * Smem::kEpiSlotBytes;
         const float* cs_row = p.cos_sin + (int64_t)__ldg(p.positions + u.r) * kD;
         const int n_rows = G + (need_epi ? 1 : 0);
         for (int base = 0; base < n_rows; base += 2) {
@@ -311,7 +338,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
                       : *reinterpret_cast<const Vec8*>(p.q + (int64_t)u.r * p.q_rs + (int64_t)(u.h * G + g) * kD + cc * 8);
           const Vec8 rv = qknorm_rope_lanes<T, 16, true>(xv, cc, is_k ? p.kw : p.qw, p.eps, cs_row, active);
           if (active) {
-            if (!is_k && need_q) *reinterpret_cast<Vec8*>(qdst + (cc >> 3) * 1024 + sw128_offset(g, cc & 7)) = rv;
+            if (!is_k && need_q) *reinterpret_cast<Vec8*>(qdst + (cc >> 3) * Smem::kQHalfBytes + sw128_offset(g, cc & 7)) = rv;
             if (need_epi) *reinterpret_cast<Vec8*>(edst + g * (kD * 2) + cc * 16) = rv;
           }
         }
@@ -332,38 +359,44 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     T* const tsel = nullptr;        // selects the bf16 / fp16 wgmma overload
     const int ct = tid - 128;       // 0..127
     const int cw = warp - 4;        // warp of the group
-    // accumulator fragment (see sm90.cuh): element i of 64-row block mb is row mb*64 + r0 + (i>>1)*8,
-    // column h0 + (i&1).  Rows are keys (S^T) or head dims (O^T), columns are the group's query heads.
+    // accumulator fragment (see sm90.cuh): element i of 64-row block mb is row mb*64 + r0 + ((i>>1)&1)*8,
+    // column (i>>2)*8 + h0 + (i&1).  Rows are keys (S^T) or head dims (O^T), columns are the group's query
+    // heads.  A thread owns kE columns; column slot e is column col_of(e), fragment element i is in slot_of(i).
     const int r0 = 16 * cw + (lane >> 2), h0 = 2 * (lane & 3);
-    auto row_of = [&](int mb, int i) { return mb * 64 + r0 + ((i >> 1) << 3); };
-    float* red_max = red;          // [4 warps][8 heads]
-    float* red_sum0 = red + 32;    // [2 parity][4][8]
-    float* red_new0 = red + 96;    // [2 parity][4][8]
+    auto row_of = [&](int mb, int i) { return mb * 64 + r0 + (((i >> 1) & 1) << 3); };
+    auto col_of = [&](int e) { return (e >> 1) * 8 + h0 + (e & 1); };
+    auto slot_of = [](int i) { return ((i >> 2) << 1) | (i & 1); };
+    float* red_max = red;            // [4 warps][N heads]
+    float* red_sum0 = red + 4 * N;   // [2 parity][4][N]
+    float* red_new0 = red + 12 * N;  // [2 parity][4][N]
     RingCursor<kStages> kv;
     RingCursor<2> qr;
     RingCursor<kFinRing> fr;
-    RingCursor<kEpiSlots> er;
+    RingCursor<Smem::kEpiSlots> er;
     uint32_t unit_par = 0;
     for (int k = 0; k < units.n_rounds; ++k) {
       const Unit u = units.at(k);
       if (units.none(u)) continue;
-      float acc[2][4], l_thr[2], m_run[2];
+      float acc[2][N / 2], l_thr[kE], m_run[kE];
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
+      for (int e = 0; e < kE; ++e) {
         l_thr[e] = 0.f;
         m_run[e] = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) acc[e][i] = 0.f;
       }
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) acc[mb][i] = 0.f;
       // operands of the appended token's score / value (x = mb*2 + (i>>1) indexes this thread's four dims):
       // issue the loads now, use them in the epilogue -- their latency hides behind the tile loop
-      float q_new[2][4], kn[4], vn[4];
+      float q_new[kE][4], kn[4], vn[4];
       int app_loc = 0;
       Vec8 app_x = Vec8{{0u, 0u, 0u, 0u}};
 #pragma unroll
       for (int x = 0; x < 4; ++x) {
         kn[x] = vn[x] = 0.f;
-        q_new[0][x] = q_new[1][x] = 0.f;
+#pragma unroll
+        for (int e = 0; e < kE; ++e) q_new[e][x] = 0.f;
       }
       if (u.last_chunk) {
 #pragma unroll
@@ -371,9 +404,9 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           const int dim = row_of(x >> 1, (x & 1) << 1);
           if (!p.fuse) {  // fused mode: roped q / k come from the Q loader's ring in the epilogue
 #pragma unroll
-            for (int e = 0; e < 2; ++e)
-              if (h0 + e < G)
-                q_new[e][x] = DTypeTraits<T>::to_float(p.q[(int64_t)u.r * p.q_rs + (int64_t)(u.h * G + h0 + e) * kD + dim]);
+            for (int e = 0; e < kE; ++e)
+              if (col_of(e) < G)
+                q_new[e][x] = DTypeTraits<T>::to_float(p.q[(int64_t)u.r * p.q_rs + (int64_t)(u.h * G + h0 + (e & 1) + (e >> 1) * 8) * kD + dim]);
             kn[x] = DTypeTraits<T>::to_float(p.k_new[(int64_t)u.r * p.k_rs + u.h * kD + dim]);
           }
           vn[x] = DTypeTraits<T>::to_float(p.v_new[(int64_t)u.r * p.v_rs + u.h * kD + dim]);
@@ -389,25 +422,25 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       if (u.n_tiles > 0) {
         const uint32_t qb = qr.stage();
         qr.wait_full(bar(kQFull));
-        const uint32_t qa = sbase + Smem::qbuf + qb * kQBufBytes;
+        const uint32_t qa = sbase + Smem::qbuf + qb * Smem::kQBufBytes;
         for (int j = 0; j < u.n_tiles; ++j, kv.advance()) {
           const uint32_t stage = kv.stage();
-          // ---- S^T = K_tile . Q^T: A = K rows (K-major, 128B swizzle), B = Q rows (K-major)
+          // ---- S^T = K_tile . Q^T: A = K rows (K-major, 128B swizzle), B = Q rows (K-major, 8-row atoms 1024 B apart)
           kv.wait_full(bar(kFullK));
           const uint32_t kb = sbase + Smem::kring + stage * kKvTileBytes;
-          float s[2][4];
+          float s[2][N / 2];
 #pragma unroll
           for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) s[mb][i] = 0.f;
+            for (int i = 0; i < N / 2; ++i) s[mb][i] = 0.f;
           wgmma_fence();
 #pragma unroll
           for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
             for (int kk = 0; kk < 8; ++kk) {
               const uint64_t da = make_smem_desc(kb + mb * 8192 + (kk >> 2) * kKvHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
-              const uint64_t db = make_smem_desc(qa + (kk >> 2) * 1024 + (kk & 3) * 32, 16, 1024, kLayoutSW128);
-              wgmma_m64n8k16_ss<0>(s[mb], da, db, kk > 0, tsel);
+              const uint64_t db = make_smem_desc(qa + (kk >> 2) * Smem::kQHalfBytes + (kk & 3) * 32, 16, 1024, kLayoutSW128);
+              wgmma_ss<N, 0>(s[mb], da, db, kk > 0, tsel);
             }
           wgmma_commit();
           wgmma_wait0();
@@ -430,49 +463,55 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             fence_proxy_async_smem();
           }
           // ---- online softmax: per head (column) max over the 128 keys of the tile
-          float mx[2] = {-INFINITY, -INFINITY};
+          float mx[kE];
+#pragma unroll
+          for (int e = 0; e < kE; ++e) mx[e] = -INFINITY;
 #pragma unroll
           for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
+            for (int i = 0; i < N / 2; ++i) {
               const float v = row_of(mb, i) < n_valid ? s[mb][i] * p.scale_log2 : -INFINITY;
               s[mb][i] = v;
-              mx[i & 1] = fmaxf(mx[i & 1], v);
+              mx[slot_of(i)] = fmaxf(mx[slot_of(i)], v);
             }
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
+          for (int e = 0; e < kE; ++e) {
             mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 4));
             mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 8));
             mx[e] = fmaxf(mx[e], __shfl_xor_sync(0xffffffffu, mx[e], 16));
           }
           if (lane < 4) {
-            red_max[cw * 8 + h0] = mx[0];
-            red_max[cw * 8 + h0 + 1] = mx[1];
+#pragma unroll
+            for (int e = 0; e < kE; ++e) red_max[cw * N + col_of(e)] = mx[e];
           }
           named_bar_sync(1, 128);
-          float alpha[2], psum[2] = {0.f, 0.f};
+          float alpha[kE], psum[kE];
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int hh = h0 + e;
-            const float mt = fmaxf(fmaxf(red_max[hh], red_max[8 + hh]), fmaxf(red_max[16 + hh], red_max[24 + hh]));
+          for (int e = 0; e < kE; ++e) {
+            const int hh = col_of(e);
+            const float mt = fmaxf(fmaxf(red_max[hh], red_max[N + hh]), fmaxf(red_max[2 * N + hh], red_max[3 * N + hh]));
             const float m_new = fmaxf(m_run[e], mt);  // finite: every tile has >= 1 valid key
             alpha[e] = fast_exp2(m_run[e] - m_new);
             m_run[e] = m_new;
+            psum[e] = 0.f;
           }
-          // P^T [head][key] as 8x8 core matrices (no swizzle, K-major): key chunks of 8 are 128 B apart
+          // P^T [head][key] as 8x8 core matrices (no swizzle, K-major): key chunks of 8 are 128 B apart, and at
+          // N = 16 heads 8-15 follow heads 0-7 as a second [8 x 128] block (kPBlockBytes)
           uint8_t* pdst = smem + Smem::pbuf;
+          constexpr int kPBlockBytes = 8 * kKvTileRows * 2;
 #pragma unroll
           for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int key = row_of(mb, i), hh = h0 + (i & 1);
-              const float pv = fast_exp2(s[mb][i] - m_run[i & 1]);
-              psum[i & 1] += pv;
-              *reinterpret_cast<T*>(pdst + (key >> 3) * 128 + hh * 16 + (key & 7) * 2) = DTypeTraits<T>::from_float(pv);
-              acc[mb][i] *= alpha[i & 1];
+            for (int i = 0; i < N / 2; ++i) {
+              const int key = row_of(mb, i), hh = h0 + (i & 1), e = slot_of(i);
+              const float pv = fast_exp2(s[mb][i] - m_run[e]);
+              psum[e] += pv;
+              *reinterpret_cast<T*>(pdst + (i >> 2) * kPBlockBytes + (key >> 3) * 128 + hh * 16 + (key & 7) * 2) =
+                  DTypeTraits<T>::from_float(pv);
+              acc[mb][i] *= alpha[e];
             }
 #pragma unroll
-          for (int e = 0; e < 2; ++e) l_thr[e] = l_thr[e] * alpha[e] + psum[e];
+          for (int e = 0; e < kE; ++e) l_thr[e] = l_thr[e] * alpha[e] + psum[e];
           fence_proxy_async_smem();  // P^T (and zeroed V rows) visible to the tensor core
           named_bar_sync(1, 128);    // every warp's P^T is written; the tile maxima may be overwritten
           // ---- O^T += V_tile^T . P^T: A = V rows read MN-major, B = P^T (K-major, no swizzle)
@@ -486,8 +525,9 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             for (int kk = 0; kk < 8; ++kk) {
               // 16 keys = two 8-key swizzle atoms of 1024 B; dims 64..127 in the second half (+16 KB)
               const uint64_t da = make_smem_desc(vb + mb * kKvHalfBytes + kk * 2048, kKvHalfBytes, 1024, kLayoutSW128);
-              const uint64_t db = make_smem_desc(pb + kk * 256, 128, 1024, kLayoutNone);
-              wgmma_m64n8k16_ss<kTransV ? 1 : 0>(acc[mb], da, db, 1u, tsel);
+              // P^T: LBO = 128 B between key chunks; SBO = the head-block stride (unused at N = 8: one block)
+              const uint64_t db = make_smem_desc(pb + kk * 256, 128, N == 8 ? 1024 : kPBlockBytes, kLayoutNone);
+              wgmma_ss<N, kTransV ? 1 : 0>(acc[mb], da, db, 1u, tsel);
             }
           wgmma_commit();
           wgmma_wait0();
@@ -500,8 +540,8 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       // ---- unit epilogue on CUDA cores: row sums, the appended token (score, value, pool append), output.
       // Reduction scratch double buffered by unit parity: the next unit may write its slots while
       // stragglers still read this unit's (every unit passes a named barrier in between).
-      float* red_sum = red_sum0 + unit_par * 32;
-      float* red_new = red_new0 + unit_par * 32;
+      float* red_sum = red_sum0 + unit_par * (4 * N);
+      float* red_new = red_new0 + unit_par * (4 * N);
       unit_par ^= 1;
       const bool epi = p.fuse && u.last_chunk;
       const uint32_t es = er.stage();
@@ -509,19 +549,19 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
         // fused mode: the Q loader left the roped q rows of the group and the roped new k row in the ring
         er.wait_full(bar(kEpiFull));
         er.advance();
-        const uint8_t* esrc = smem + Smem::epi + es * kEpiSlotBytes;
+        const uint8_t* esrc = smem + Smem::epi + es * Smem::kEpiSlotBytes;
 #pragma unroll
         for (int x = 0; x < 4; ++x) {
           const int dim = row_of(x >> 1, (x & 1) << 1);
 #pragma unroll
-          for (int e = 0; e < 2; ++e)
-            if (h0 + e < G) q_new[e][x] = DTypeTraits<T>::to_float(*reinterpret_cast<const T*>(esrc + (h0 + e) * (kD * 2) + dim * 2));
+          for (int e = 0; e < kE; ++e)
+            if (col_of(e) < G) q_new[e][x] = DTypeTraits<T>::to_float(*reinterpret_cast<const T*>(esrc + col_of(e) * (kD * 2) + dim * 2));
           kn[x] = DTypeTraits<T>::to_float(*reinterpret_cast<const T*>(esrc + G * (kD * 2) + dim * 2));
         }
         if (ct < 16) app_x = *reinterpret_cast<const Vec8*>(esrc + G * (kD * 2) + ct * 16);
       }
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
+      for (int e = 0; e < kE; ++e) {
         float ls = l_thr[e], sn = 0.f;
         if (u.last_chunk) sn = (q_new[e][0] * kn[0] + q_new[e][1] * kn[1]) + (q_new[e][2] * kn[2] + q_new[e][3] * kn[3]);
 #pragma unroll
@@ -530,30 +570,31 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           sn += __shfl_xor_sync(0xffffffffu, sn, o);
         }
         if (lane < 4) {
-          red_sum[cw * 8 + h0 + e] = ls;
-          red_new[cw * 8 + h0 + e] = sn;
+          red_sum[cw * N + col_of(e)] = ls;
+          red_new[cw * N + col_of(e)] = sn;
         }
       }
       named_bar_sync(1, 128);
       if (epi && ct == 0) mbar_arrive(bar(kEpiEmpty + es));  // every thread has read its ring values
-      float l_tot[2];
+      float l_tot[kE];
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int hh = h0 + e;
-        l_tot[e] = red_sum[hh] + red_sum[8 + hh] + red_sum[16 + hh] + red_sum[24 + hh];
+      for (int e = 0; e < kE; ++e) {
+        const int hh = col_of(e);
+        l_tot[e] = red_sum[hh] + red_sum[N + hh] + red_sum[2 * N + hh] + red_sum[3 * N + hh];
       }
       if (u.last_chunk) {
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int hh = h0 + e;
-          const float s_new = (red_new[hh] + red_new[8 + hh] + red_new[16 + hh] + red_new[24 + hh]) * p.scale_log2;
+        for (int e = 0; e < kE; ++e) {
+          const int hh = col_of(e);
+          const float s_new = (red_new[hh] + red_new[N + hh] + red_new[2 * N + hh] + red_new[3 * N + hh]) * p.scale_log2;
           const float m_new = fmaxf(m_run[e], s_new);
           const float a = fast_exp2(m_run[e] - m_new);
           const float pnew = fast_exp2(s_new - m_new);
+          const int i0 = (e >> 1) * 4 + (e & 1);  // fragment elements of column slot e: i0 (row r0), i0 + 2 (row r0 + 8)
 #pragma unroll
           for (int mb = 0; mb < 2; ++mb) {
-            acc[mb][e] = acc[mb][e] * a + pnew * vn[mb * 2];
-            acc[mb][2 + e] = acc[mb][2 + e] * a + pnew * vn[mb * 2 + 1];
+            acc[mb][i0] = acc[mb][i0] * a + pnew * vn[mb * 2];
+            acc[mb][i0 + 2] = acc[mb][i0 + 2] * a + pnew * vn[mb * 2 + 1];
           }
           l_tot[e] = l_tot[e] * a + pnew;
           m_run[e] = m_new;
@@ -566,28 +607,30 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       }
       // ---- write out
       if (u.n_chunks == 1) {
-        const float inv[2] = {1.f / l_tot[0], 1.f / l_tot[1]};
+        float inv[kE];
+#pragma unroll
+        for (int e = 0; e < kE; ++e) inv[e] = 1.f / l_tot[e];
 #pragma unroll
         for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
-            if (h0 + (i & 1) < G)
-              p.out[((int64_t)u.r * p.hq + u.h * G + h0 + (i & 1)) * kD + row_of(mb, i)] =
-                  DTypeTraits<T>::from_float(acc[mb][i] * inv[i & 1]);
+          for (int i = 0; i < N / 2; ++i)
+            if (col_of(slot_of(i)) < G)
+              p.out[((int64_t)u.r * p.hq + u.h * G + h0 + (i & 1) + (i >> 2) * 8) * kD + row_of(mb, i)] =
+                  DTypeTraits<T>::from_float(acc[mb][i] * inv[slot_of(i)]);
       } else {
         const int64_t base = ((int64_t)u.r * kMaxSplits + u.c) * p.hq + u.h * G;
 #pragma unroll
         for (int mb = 0; mb < 2; ++mb)
 #pragma unroll
-          for (int i = 0; i < 4; ++i)
-            if (h0 + (i & 1) < G) p.part_o[(base + h0 + (i & 1)) * kD + row_of(mb, i)] = acc[mb][i];
+          for (int i = 0; i < N / 2; ++i)
+            if (col_of(slot_of(i)) < G) p.part_o[(base + h0 + (i & 1) + (i >> 2) * 8) * kD + row_of(mb, i)] = acc[mb][i];
         if (cw == 0 && lane < 4) {
-          // m_run / l_tot of a head are uniform across threads; lanes 0-3 of warp 0 store heads h0, h0+1
+          // m_run / l_tot of a head are uniform across threads; lanes 0-3 of warp 0 store their kE heads
 #pragma unroll
-          for (int e = 0; e < 2; ++e)
-            if (h0 + e < G) {
-              p.part_ml[(base + h0 + e) * 2 + 0] = m_run[e];
-              p.part_ml[(base + h0 + e) * 2 + 1] = l_tot[e];
+          for (int e = 0; e < kE; ++e)
+            if (col_of(e) < G) {
+              p.part_ml[(base + h0 + (e & 1) + (e >> 1) * 8) * 2 + 0] = m_run[e];
+              p.part_ml[(base + h0 + (e & 1) + (e >> 1) * 8) * 2 + 1] = l_tot[e];
             }
         }
         // ---- hand the unit to the combiner warp (asynchronous split-KV merge): the consumer warps
@@ -623,62 +666,70 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
         last = __shfl_sync(0xffffffffu, last, 0);
         if (last) {
           __threadfence();  // acquire the other chunks' partials
-          // The merge is pure latency (partials sit in L2, written by other SMs): every load whose address
-          // is known is issued before anything is consumed -- (m, l) of all G heads at once, then the
-          // partial outputs kMergeBatch chunks x G heads at a time.
-          const int64_t b0 = ((int64_t)u.r * kMaxSplits) * p.hq + u.h * G;
-          float mc[G], lc[G];
+          // Heads in passes of GB <= 8: (o, m, l, weight, 1/l) of 9-16 heads plus their prefetched partials would
+          // not fit one warp's registers.  A group of 9-15 ends its last pass at head G-1, so that pass merges some
+          // heads of the first one again -- with the same bits, as a head's merge reads only its own partials.
+          constexpr int GB = G <= 8 ? G : 8;
 #pragma unroll
-          for (int g = 0; g < G; ++g) {  // lane c holds (m, l) of chunk c
-            mc[g] = -INFINITY;
-            lc[g] = 0.f;
-            if (lane < u.n_chunks) {
-              const float2 ml = __ldcg(reinterpret_cast<const float2*>(p.part_ml + (b0 + (int64_t)lane * p.hq + g) * 2));
-              mc[g] = ml.x;
-              lc[g] = ml.y;
-            }
-          }
-          constexpr int kMergeBatch = G <= 2 ? 8 : (G <= 4 ? 4 : 2);
-          float4 o[G];
-          float wc[G], inv[G];
+          for (int pass = 0; pass < (G + GB - 1) / GB; ++pass) {
+            const int g0 = min(pass * GB, G - GB);  // first head of the pass
+            // The merge is pure latency (partials sit in L2, written by other SMs): every load whose address
+            // is known is issued before anything is consumed -- (m, l) of all GB heads at once, then the
+            // partial outputs kMergeBatch chunks x GB heads at a time.
+            const int64_t b0 = ((int64_t)u.r * kMaxSplits) * p.hq + u.h * G + g0;
+            float mc[GB], lc[GB];
 #pragma unroll
-          for (int g = 0; g < G; ++g) o[g] = make_float4(0.f, 0.f, 0.f, 0.f);
-          for (int c0 = 0; c0 < u.n_chunks; c0 += kMergeBatch) {
-            float4 po[G][kMergeBatch];
-#pragma unroll
-            for (int g = 0; g < G; ++g)
-#pragma unroll
-              for (int j = 0; j < kMergeBatch; ++j)
-                po[g][j] = c0 + j < u.n_chunks
-                               ? __ldcg(reinterpret_cast<const float4*>(p.part_o + (b0 + (int64_t)(c0 + j) * p.hq + g) * kD) + lane)
-                               : make_float4(0.f, 0.f, 0.f, 0.f);
-            if (c0 == 0) {
-#pragma unroll
-              for (int g = 0; g < G; ++g) {
-                const float mx = warp_max(mc[g]);
-                wc[g] = lane < u.n_chunks ? fast_exp2(mc[g] - mx) : 0.f;
-                inv[g] = 1.f / warp_sum(wc[g] * lc[g]);
+            for (int g = 0; g < GB; ++g) {  // lane c holds (m, l) of chunk c
+              mc[g] = -INFINITY;
+              lc[g] = 0.f;
+              if (lane < u.n_chunks) {
+                const float2 ml = __ldcg(reinterpret_cast<const float2*>(p.part_ml + (b0 + (int64_t)lane * p.hq + g) * 2));
+                mc[g] = ml.x;
+                lc[g] = ml.y;
               }
             }
+            constexpr int kMergeBatch = GB <= 2 ? 8 : (GB <= 4 ? 4 : 2);
+            float4 o[GB];
+            float wc[GB], inv[GB];
 #pragma unroll
-            for (int g = 0; g < G; ++g)
+            for (int g = 0; g < GB; ++g) o[g] = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int c0 = 0; c0 < u.n_chunks; c0 += kMergeBatch) {
+              float4 po[GB][kMergeBatch];
 #pragma unroll
-              for (int j = 0; j < kMergeBatch; ++j) {  // chunk order 0, 1, ... as in combine.cuh
-                const float w = __shfl_sync(0xffffffffu, wc[g], (c0 + j) & 31);
-                o[g].x += w * po[g][j].x;
-                o[g].y += w * po[g][j].y;
-                o[g].z += w * po[g][j].z;
-                o[g].w += w * po[g][j].w;
+              for (int g = 0; g < GB; ++g)
+#pragma unroll
+                for (int j = 0; j < kMergeBatch; ++j)
+                  po[g][j] = c0 + j < u.n_chunks
+                                 ? __ldcg(reinterpret_cast<const float4*>(p.part_o + (b0 + (int64_t)(c0 + j) * p.hq + g) * kD) + lane)
+                                 : make_float4(0.f, 0.f, 0.f, 0.f);
+              if (c0 == 0) {
+#pragma unroll
+                for (int g = 0; g < GB; ++g) {
+                  const float mx = warp_max(mc[g]);
+                  wc[g] = lane < u.n_chunks ? fast_exp2(mc[g] - mx) : 0.f;
+                  inv[g] = 1.f / warp_sum(wc[g] * lc[g]);
+                }
               }
-          }
 #pragma unroll
-          for (int g = 0; g < G; ++g) {
-            typename DTypeTraits<T>::T2 lo = DTypeTraits<T>::from_float2(o[g].x * inv[g], o[g].y * inv[g]);
-            typename DTypeTraits<T>::T2 hi = DTypeTraits<T>::from_float2(o[g].z * inv[g], o[g].w * inv[g]);
-            uint2 pk;
-            pk.x = *reinterpret_cast<uint32_t*>(&lo);
-            pk.y = *reinterpret_cast<uint32_t*>(&hi);
-            *reinterpret_cast<uint2*>(p.out + ((int64_t)u.r * p.hq + u.h * G + g) * kD + lane * 4) = pk;
+              for (int g = 0; g < GB; ++g)
+#pragma unroll
+                for (int j = 0; j < kMergeBatch; ++j) {  // chunk order 0, 1, ... as in combine.cuh
+                  const float w = __shfl_sync(0xffffffffu, wc[g], (c0 + j) & 31);
+                  o[g].x += w * po[g][j].x;
+                  o[g].y += w * po[g][j].y;
+                  o[g].z += w * po[g][j].z;
+                  o[g].w += w * po[g][j].w;
+                }
+            }
+#pragma unroll
+            for (int g = 0; g < GB; ++g) {
+              typename DTypeTraits<T>::T2 lo = DTypeTraits<T>::from_float2(o[g].x * inv[g], o[g].y * inv[g]);
+              typename DTypeTraits<T>::T2 hi = DTypeTraits<T>::from_float2(o[g].z * inv[g], o[g].w * inv[g]);
+              uint2 pk;
+              pk.x = *reinterpret_cast<uint32_t*>(&lo);
+              pk.y = *reinterpret_cast<uint32_t*>(&hi);
+              *reinterpret_cast<uint2*>(p.out + ((int64_t)u.r * p.hq + u.h * G + g0 + g) * kD + lane * 4) = pk;
+            }
           }
         }
         __syncwarp();
@@ -695,7 +746,7 @@ template <typename T, int G>
 static int launch_g(const Params<T>& p, const CUtensorMap& mk, const CUtensorMap& mv,
                     const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& tk,
                     const CUtensorMap& tv, cudaStream_t st) {
-  const size_t smem = Smem::total + 1024;
+  const size_t smem = Smem<kNOf<G>>::total + 1024;
   static bool configured = false;
   if (!configured) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(attn_decode_tc_kernel<T, G>,
@@ -749,8 +800,17 @@ static int launch(const DecodeArgs& a) {
     case 6: return launch_g<T, 6>(p, mk, mv, bk, bv, tk, tv, a.stream);
     case 7: return launch_g<T, 7>(p, mk, mv, bk, bv, tk, tv, a.stream);
     case 8: return launch_g<T, 8>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    default:
-      set_error("attn_decode: GQA group size %d not supported (1..8)", p.hq / p.hkv);
+    case 9: return launch_g<T, 9>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 10: return launch_g<T, 10>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 11: return launch_g<T, 11>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 12: return launch_g<T, 12>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 13: return launch_g<T, 13>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 14: return launch_g<T, 14>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 15: return launch_g<T, 15>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 16: return launch_g<T, 16>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    default:  // attn_decode() has refused every other group size
+      set_error("attn_decode: GQA group size %d not supported by the wgmma decode kernel (1..%d)", p.hq / p.hkv,
+                kMaxGroup);
       return 1;
   }
 }
@@ -784,9 +844,17 @@ static int attn_decode(const DecodeArgs& a) {
                  (long long)a.num_slots);
   B200_CHECK_ARG(a.st_stride % 4 == 0 && ((uintptr_t)a.slot_table % 16) == 0,
                  "attn_decode: slot table rows must be 16-byte aligned");
-  if (g_decode_impl.load() == 1)
+  const int group = a.hq / a.hkv;
+  if (g_decode_impl.load() == 1) {
+    B200_CHECK_ARG(group <= dtc::kMaxGroup,
+                   "attn_decode: GQA group size %d (hq/hkv) not supported by the wgmma decode kernel (1..%d)", group,
+                   dtc::kMaxGroup);
     return a.dtype == B200_DTYPE_BF16 ? dtc::launch<__nv_bfloat16>(a) : dtc::launch<__half>(a);
+  }
   B200_CHECK_ARG(!a.fuse, "attn_decode_fused: only the wgmma kernel (decode_impl = 1) fuses qk-norm + RoPE");
+  B200_CHECK_ARG(group <= 8,
+                 "attn_decode: GQA group size %d (hq/hkv) not supported by the cp.async bring-up decode kernel (1..8)",
+                 group);
 #ifdef B200_BRINGUP_KERNELS
   return launch_decode_bringup(a);
 #else
