@@ -8,17 +8,22 @@ Two ways to use them:
 * inside mini-sglang: :func:`patch_minisgl_layers` re-binds the kernel attributes the reference's
   layer objects already hold (``RMSNorm.rmsnorm`` norm.py:14, ``RMSNormFused.{rmsnorm,
   fused_add_rmsnorm}`` norm.py:29-30, ``RotaryEmbedding.apply_rope_with_cos_sin_cache_inplace``
-  rotary.py:35-37) -- zero edits to the reference.
+  rotary.py:35-37), and :func:`patch_minisgl_attention` re-binds ``forward`` of the reference's
+  ``AttentionLayer`` to :func:`attention_forward`, the same code our ``AttentionLayer`` runs -- zero
+  edits to the reference.
 """
 
 from __future__ import annotations
 
+import functools
 import math
 from typing import Any, Callable, Dict, Optional, Tuple
 
 import torch
 
 from . import ops
+from .attention.backend import B200AttnBackend
+from .attention.base import HybridBackend
 from .core import get_global_ctx
 from .utils import div_even, get_tp_info
 
@@ -127,10 +132,10 @@ class RotaryEmbedding:
 class AttentionLayer:
     """split -> q/k norm -> RoPE -> ``ctx.attn_backend.forward`` (attention.py:18-57).
 
-    ``fuse_pre_attention=True``: decode batches run norm + RoPE + KV append + attention as ONE launch
-    (``b200_attn_decode_fused``); prefill batches run the norm+RoPE sequence as a single fused launch
-    (``b200_qknorm_rope_inplace``) in front of the attention launch.  Results are bit-identical to the
-    reference's three-launch sequence followed by attention.
+    ``fuse_pre_attention=True`` runs :func:`attention_forward`: decode batches run norm + RoPE + KV append +
+    attention as ONE launch (``b200_attn_decode_fused``); prefill batches run the norm+RoPE sequence as a
+    single fused launch (``b200_qknorm_rope_inplace``) in front of the attention launch.  Results are
+    bit-identical to the reference's three-launch sequence followed by attention.
     """
 
     def __init__(
@@ -159,50 +164,91 @@ class AttentionLayer:
         self.fuse_pre_attention = fuse_pre_attention
 
     def forward(self, qkv: torch.Tensor) -> torch.Tensor:
+        if self.fuse_pre_attention:
+            return attention_forward(self, qkv)
         ctx = get_global_ctx()
         q, k, v = qkv.split([self.qo_attn_dim, self.kv_attn_dim, self.kv_attn_dim], dim=-1)
-        eps = self.q_norm.eps if self.q_norm is not None else (
-            self.k_norm.eps if self.k_norm is not None else 0.0
-        )
-        fused_decode = getattr(ctx.attn_backend, "forward_decode_fused", None)
-        if (self.fuse_pre_attention and fused_decode is not None and ctx.batch.is_decode
-                and ctx.batch.positions.dtype == torch.int32):
-            # decode: norm + RoPE + append + attention are ONE launch (q / k stay raw in memory)
-            o = fused_decode(
-                q.view(-1, self.num_qo_heads, self.head_dim), k, v, self.layer_id, ctx.batch,
-                ctx.batch.positions, self.rotary._cos_sin_cache,
-                self.q_norm.weight if self.q_norm is not None else None,
-                self.k_norm.weight if self.k_norm is not None else None, eps,
-            )
-            return o.view(-1, self.qo_attn_dim)
-        if self.fuse_pre_attention:
-            ops.qknorm_rope_inplace(
-                ctx.batch.positions, q, k, self.head_dim, self.rotary._cos_sin_cache,
-                self.q_norm.weight if self.q_norm is not None else None,
-                self.k_norm.weight if self.k_norm is not None else None,
-                eps,
-            )
-        else:
-            if self.q_norm is not None:
-                self.q_norm.forward_inplace(q.view(-1, self.num_qo_heads, self.head_dim))
-            if self.k_norm is not None:
-                self.k_norm.forward_inplace(k.view(-1, self.num_kv_heads, self.head_dim))
-            q, k = self.rotary.forward(ctx.batch.positions, q, k)
+        if self.q_norm is not None:
+            self.q_norm.forward_inplace(q.view(-1, self.num_qo_heads, self.head_dim))
+        if self.k_norm is not None:
+            self.k_norm.forward_inplace(k.view(-1, self.num_kv_heads, self.head_dim))
+        q, k = self.rotary.forward(ctx.batch.positions, q, k)
         q = q.view(-1, self.num_qo_heads, self.head_dim)
         o = ctx.attn_backend.forward(q, k, v, self.layer_id, ctx.batch)
         return o.view(-1, self.qo_attn_dim)
 
 
-def patch_minisgl_layers(model: Any) -> int:
-    """Re-bind the kernel attributes of every reference norm / rotary layer found under ``model``
-    (any object graph of ``BaseOP``s) to the sm_90a ops.  Returns the number of re-bound layers."""
-    seen, count = set(), 0
+def serving_attn_backend(backend: Any, batch: Any) -> Any:
+    """The backend that runs ``batch``: a ``HybridBackend`` (``--attn p,d``) hands prefill batches to its
+    ``prefill_backend`` and every other batch to its ``decode_backend`` (reference attention/base.py:45-50)."""
+    if isinstance(backend, HybridBackend):
+        return backend.prefill_backend if batch.is_prefill else backend.decode_backend
+    return backend
+
+
+def attention_forward(
+    layer: Any, qkv: torch.Tensor, unfused: Optional[Callable[[torch.Tensor], torch.Tensor]] = None
+) -> torch.Tensor:
+    """``AttentionLayer.forward`` with the pre-attention work fused into the sm_90a launches, for our
+    :class:`AttentionLayer` and for the reference's (``layer`` needs ``layer_id``, ``head_dim``,
+    ``num_qo_heads``, ``num_kv_heads``, ``qo_attn_dim``, ``kv_attn_dim``, ``rotary._cos_sin_cache`` and
+    ``q_norm`` / ``k_norm`` with ``.weight`` and ``.eps``, or None).
+
+    When the backend serving this batch is a :class:`B200AttnBackend`, a decode batch with int32 positions
+    runs q-norm + k-norm + RoPE + KV append + attention as ONE launch (``forward_decode_fused``) and every
+    other batch runs ``ops.qknorm_rope_inplace`` (one launch) and then the backend's ``forward``.  Results are
+    bit-identical to the reference's three-launch sequence followed by attention.  With any other backend
+    ``unfused(qkv)`` is returned when given; without it the fused norm + RoPE launch feeds that backend."""
+    ctx = get_global_ctx()
+    batch = ctx.batch
+    backend = serving_attn_backend(ctx.attn_backend, batch)
+    is_b200 = isinstance(backend, B200AttnBackend)
+    if unfused is not None and not is_b200:
+        return unfused(qkv)
+    q, k, v = qkv.split([layer.qo_attn_dim, layer.kv_attn_dim, layer.kv_attn_dim], dim=-1)
+    q_norm, k_norm = layer.q_norm, layer.k_norm
+    eps = q_norm.eps if q_norm is not None else (k_norm.eps if k_norm is not None else 0.0)
+    q_weight = q_norm.weight if q_norm is not None else None
+    k_weight = k_norm.weight if k_norm is not None else None
+    cos_sin_cache = layer.rotary._cos_sin_cache
+    if is_b200 and batch.is_decode and batch.positions.dtype == torch.int32:
+        # decode: norm + RoPE + append + attention are ONE launch (q / k stay raw in memory)
+        o = backend.forward_decode_fused(
+            q.view(-1, layer.num_qo_heads, layer.head_dim), k, v, layer.layer_id, batch, batch.positions,
+            cos_sin_cache, q_weight, k_weight, eps,
+        )
+        return o.view(-1, layer.qo_attn_dim)
+    ops.qknorm_rope_inplace(batch.positions, q, k, layer.head_dim, cos_sin_cache, q_weight, k_weight, eps)
+    o = backend.forward(q.view(-1, layer.num_qo_heads, layer.head_dim), k, v, layer.layer_id, batch)
+    return o.view(-1, layer.qo_attn_dim)
+
+
+def _walk(model: Any):
+    """Every object reachable from ``model`` (any object graph of ``BaseOP``s), each once; the children of an
+    object are read after the caller has seen it."""
+    seen = set()
     stack = [model]
     while stack:
         obj = stack.pop()
         if id(obj) in seen or isinstance(obj, (torch.Tensor, str, bytes, int, float)):
             continue
         seen.add(id(obj))
+        yield obj
+        children = []
+        if isinstance(obj, (list, tuple)):
+            children = list(obj)
+        elif isinstance(obj, dict):
+            children = list(obj.values())
+        elif hasattr(obj, "__dict__"):
+            children = [c for c in vars(obj).values() if not callable(c) or hasattr(c, "__dict__")]
+        stack.extend(children)
+
+
+def patch_minisgl_layers(model: Any) -> int:
+    """Re-bind the kernel attributes of every reference norm / rotary layer found under ``model``
+    (any object graph of ``BaseOP``s) to the sm_90a ops.  Returns the number of re-bound layers."""
+    count = 0
+    for obj in _walk(model):
         hit = False
         if callable(getattr(obj, "fused_add_rmsnorm", None)) and hasattr(obj, "weight"):
             obj.fused_add_rmsnorm = ops.fused_add_rmsnorm
@@ -216,14 +262,33 @@ def patch_minisgl_layers(model: Any) -> int:
             obj.apply_rope_with_cos_sin_cache_inplace = ops.apply_rope_with_cos_sin_cache_inplace
             hit = True
         count += int(hit)
-        children = []
-        if isinstance(obj, (list, tuple)):
-            children = list(obj)
-        elif isinstance(obj, dict):
-            children = list(obj.values())
-        elif hasattr(obj, "__dict__"):
-            children = [c for c in vars(obj).values() if not callable(c) or hasattr(c, "__dict__")]
-        stack.extend(children)
+    return count
+
+
+def patch_minisgl_attention(model: Any) -> int:
+    """Re-bind ``forward`` of every reference ``minisgl.layers.attention.AttentionLayer`` found under ``model``
+    to :func:`attention_forward`, so that with ``attention_backend="b200"`` (alone or as either half of a
+    hybrid) a decode step is ONE launch per layer (q-norm, k-norm, RoPE, KV append, attention) and a prefill
+    forward two (fused q/k-norm + RoPE, attention) instead of four and three.  Batches served by any other
+    backend go to the layer's original ``forward``, unchanged.  Zero edits to the reference: the original bound
+    method is kept on the instance as ``_b200_unfused_forward``.  Idempotent.  Returns the number of attention
+    layers that run :func:`attention_forward` afterwards (0 when the reference is not importable).
+
+    Patch before the decode graphs are captured (``install_into_minisgl`` does); on an engine that already
+    exists, only eager forwards change."""
+    try:
+        from minisgl.layers.attention import AttentionLayer as RefAttentionLayer
+    except ImportError:
+        return 0
+    count = 0
+    for obj in _walk(model):
+        if not isinstance(obj, RefAttentionLayer):
+            continue
+        if "_b200_unfused_forward" not in vars(obj):
+            unfused = obj.forward
+            obj._b200_unfused_forward = unfused
+            obj.forward = functools.partial(attention_forward, obj, unfused=unfused)
+        count += 1
     return count
 
 
@@ -251,28 +316,36 @@ def patch_flashinfer_entry_points() -> int:
     return len(table)
 
 
-def install_into_minisgl(norm_rope: bool = True, row_gather: bool = True) -> bool:
+def install_into_minisgl(norm_rope: bool = True, row_gather: bool = True, attention: bool = True) -> bool:
     """One call, before ``LLM(...)`` / ``Engine(...)``: makes the reference build its model with the sm_90a
-    norm / RoPE kernels and use the sm_90a row gather, with zero edits to the reference.
+    norm / RoPE kernels, fuse the pre-attention work of its attention layers into the b200 launches and use
+    the sm_90a row gather, with zero edits to the reference.
 
     ``Engine.__init__`` asserts that CUDA is not initialised yet (engine/engine.py:31) and importing
     ``flashinfer`` initialises it, so the FlashInfer names cannot be re-bound up front.  Instead the module
     attribute ``minisgl.engine.engine.create_model`` (engine.py:12, called at engine.py:50-51 after the device
     is set and before the decode graphs are captured at engine.py:100) is wrapped: the wrapper re-binds the
-    FlashInfer entry points (:func:`patch_flashinfer_entry_points`) and then calls the reference's own
-    ``create_model``.  Returns False when the reference is not importable."""
+    FlashInfer entry points (:func:`patch_flashinfer_entry_points`, ``norm_rope``), calls the reference's own
+    ``create_model`` and re-binds ``forward`` of the model's attention layers (:func:`patch_minisgl_attention`,
+    ``attention``).  So with ``attention_backend="b200"`` every decode step inside the engine's CUDA graphs is
+    ONE launch per layer (q-norm + k-norm + RoPE + KV append + attention); layers whose batch another backend
+    serves keep their own forward.  Returns False when the reference is not importable."""
     try:
         import minisgl.engine.engine as ref_engine
     except ImportError:
         return False
     if row_gather:
         patch_minisgl_kernels()
-    if norm_rope and not getattr(ref_engine.create_model, "_b200_wrapped", False):
+    if (norm_rope or attention) and not getattr(ref_engine.create_model, "_b200_wrapped", False):
         real_create_model = ref_engine.create_model
 
         def create_model_with_b200_layers(*args, **kwargs):
-            patch_flashinfer_entry_points()
-            return real_create_model(*args, **kwargs)
+            if norm_rope:
+                patch_flashinfer_entry_points()
+            model = real_create_model(*args, **kwargs)
+            if attention:
+                patch_minisgl_attention(model)
+            return model
 
         create_model_with_b200_layers._b200_wrapped = True  # type: ignore[attr-defined]
         ref_engine.create_model = create_model_with_b200_layers

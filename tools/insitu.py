@@ -6,9 +6,10 @@ forward (prefill, chunked prefill, radix-hit extend, graph-replayed padded decod
 
   child mode (one process per engine -- `Engine` asserts a fresh CUDA context, engine.py:32):
       python tools/insitu.py child --attn b200 --page-size 64 --out /tmp/x.pt [--force /tmp/fi.pt]
-             [--patch none|flashinfer|model] [--patch-kernels]
+             [--patch none|flashinfer|model|fused] [--patch-kernels] [--unfused-attention]
   driver mode (spawns the children, compares, prints + writes a JSON summary):
       python tools/insitu.py run --out insitu_summary.json
+  `run_fused()` spawns the children of tests/test_gpu_insitu_fused.py (`--patch fused` against `--patch model`).
 
 What the reference is asked to do (reference file:line of the code that runs):
   * `LLM.generate` twice (llm/llm.py:81-98): round A fills the radix cache, round B re-uses two of
@@ -93,22 +94,37 @@ def child(args) -> None:
 
         b200_layers = minisgl_b200.PACKAGE.layers
     if args.patch == "flashinfer":  # the documented one-call integration (INTEGRATION.md section 2)
-        assert b200_layers.install_into_minisgl(norm_rope=True, row_gather=args.patch_kernels)
+        assert b200_layers.install_into_minisgl(norm_rope=True, row_gather=args.patch_kernels,
+                                                attention=not args.unfused_attention)
     import minisgl.scheduler.scheduler as ref_sched
 
     ref_sched.load_tokenizer = lambda path: _StubTokenizer()  # no tokenizer files offline
-    if args.patch == "model":
-        import minisgl.engine.engine as ref_engine
+    import minisgl.engine.engine as ref_engine
+    from minisgl.core import get_global_ctx as ref_ctx
 
-        real_runner = ref_engine.GraphRunner
+    real_runner = ref_engine.GraphRunner
+    forwards = {"prefill": 0, "decode": 0}  # model forwards that launch kernels: eager or being captured
 
-        def runner_with_patched_model(*a, **kw):
-            n = b200_layers.patch_minisgl_layers(kw["model"])
+    def runner_with_patched_model(*a, **kw):
+        model = kw["model"]
+        if args.patch in ("model", "fused"):
+            n = b200_layers.patch_minisgl_layers(model)
             print(f"[insitu] patch_minisgl_layers re-bound {n} layers", flush=True)
             assert n > 0
-            return real_runner(*a, **kw)
+        if args.patch == "fused":
+            n = b200_layers.patch_minisgl_attention(model)
+            print(f"[insitu] patch_minisgl_attention re-bound {n} layers", flush=True)
+            assert n == args.layers
+        real_model_forward = model.forward
 
-        ref_engine.GraphRunner = runner_with_patched_model
+        def counted_forward(*fa, **fkw):  # graph replays do not call it
+            forwards[ref_ctx().batch.phase] += 1
+            return real_model_forward(*fa, **fkw)
+
+        model.forward = counted_forward
+        return real_runner(*a, **kw)
+
+    ref_engine.GraphRunner = runner_with_patched_model
     if args.patch_kernels:
         assert b200_layers.patch_minisgl_kernels()
 
@@ -190,7 +206,7 @@ def child(args) -> None:
     if uses_b200 or args.patch != "none" or args.patch_kernels:
         launches = int(minisgl_b200.PACKAGE._cabi.launch_count())
     torch.save({"records": records, "tokens": tokens_out, "append_keys": keys, "kv": kv,
-                "b200_launches": launches, "args": vars(args)}, args.out)
+                "b200_launches": launches, "forwards": forwards, "args": vars(args)}, args.out)
     print(f"[insitu] {len(records)} forwards recorded, b200 kernel launches: {launches}", flush=True)
     try:
         llm.shutdown()
@@ -259,7 +275,8 @@ def logits_bit_identical(path_a: str, path_b: str) -> bool:
 
 
 def run_child(tag: str, out_dir: Path, attn: str, page_size: int, force: "str | None", patch: str = "none",
-              patch_kernels: bool = False, layers: int = 28, timeout: int = 600, fi_tensor_cores: bool = False) -> str:
+              patch_kernels: bool = False, layers: int = 28, timeout: int = 600, fi_tensor_cores: bool = False,
+              unfused_attention: bool = False) -> str:
     out = out_dir / f"{tag}.pt"
     cmd = [sys.executable, str(Path(__file__).resolve()), "child", "--attn", attn, "--page-size", str(page_size),
            "--out", str(out), "--patch", patch, "--layers", str(layers)]
@@ -269,6 +286,8 @@ def run_child(tag: str, out_dir: Path, attn: str, page_size: int, force: "str | 
         cmd += ["--patch-kernels"]
     if fi_tensor_cores:
         cmd += ["--fi-tensor-cores"]
+    if unfused_attention:
+        cmd += ["--unfused-attention"]
     t0 = time.time()
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=timeout, cwd=str(ROOT))
     log = res.stdout.decode(errors="replace")
@@ -328,6 +347,32 @@ def run(args) -> dict:
     return summary
 
 
+def run_fused(args) -> dict:
+    """The fused attention forward inside the engine (`patch_minisgl_attention`, `--patch fused`) next to the
+    unfused patched model (`--patch model`, our norm / RoPE kernels as separate launches) at page sizes 64 and 1,
+    the one-call `install_into_minisgl` with the b200 backend, and with the reference's own fi backend with and
+    without the attention patch.  Every run is teacher-forced with the tokens of the free-running fi_p64 run.
+    Returns {tag: path of the child's .pt}; the comparisons are the caller's (tests/test_gpu_insitu_fused.py)."""
+    out_dir = Path(tempfile.mkdtemp(prefix="insitu_fused_"))
+    L = args.layers
+    fi64 = run_child("fi_p64", out_dir, "fi", 64, None, layers=L)
+    runs = {"fi_p64": fi64}
+    plan = [
+        ("fi_tc_p64", dict(attn="fi", page_size=64, fi_tensor_cores=True)),
+        ("b200_p64_patched", dict(attn="b200", page_size=64, patch="model", patch_kernels=True)),
+        ("b200_p64_fused", dict(attn="b200", page_size=64, patch="fused", patch_kernels=True)),
+        ("b200_p1_patched", dict(attn="b200", page_size=1, patch="model", patch_kernels=True)),
+        ("b200_p1_fused", dict(attn="b200", page_size=1, patch="fused", patch_kernels=True)),
+        ("b200_p64_installed", dict(attn="b200", page_size=64, patch="flashinfer", patch_kernels=True)),
+        ("fi_p64_installed", dict(attn="fi", page_size=64, patch="flashinfer", patch_kernels=True)),
+        ("fi_p64_installed_unfused", dict(attn="fi", page_size=64, patch="flashinfer", patch_kernels=True,
+                                          unfused_attention=True)),
+    ]
+    for tag, kw in plan:
+        runs[tag] = run_child(tag, out_dir, force=fi64, layers=L, **kw)
+    return runs
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     sub = ap.add_subparsers(dest="mode", required=True)
@@ -339,7 +384,9 @@ def main() -> None:
     c.add_argument("--layers", type=int, default=28)
     c.add_argument("--out", required=True)
     c.add_argument("--force", default=None)
-    c.add_argument("--patch", default="none", choices=["none", "flashinfer", "model"])
+    c.add_argument("--patch", default="none", choices=["none", "flashinfer", "model", "fused"])
+    c.add_argument("--unfused-attention", action="store_true",
+                   help="--patch flashinfer: install_into_minisgl(attention=False)")
     c.add_argument("--patch-kernels", action="store_true")
     c.add_argument("--fi-tensor-cores", action="store_true")
     r = sub.add_parser("run")
