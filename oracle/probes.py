@@ -1,8 +1,9 @@
 """Exact-answer probes of the attention kernels and an fp64 softmax reference with an element-wise error
 bound (TEST INFRASTRUCTURE ONLY: imported by tests/).
 
-Needle.  Query head (h, g) (kv head h, slot g < 8 of its GQA group) has q[g] = 32 and zeros in every other
-dim; its chosen key p has K[p, h, g] = 64 and every other key has zeros in dims 0-9.  The needle scores
+Needle.  Query head (h, g) (kv head h, slot g < 16 of its GQA group) has q[needle_dim(g)] = 32 and zeros in
+every other dim (needle_dim: dims 0-7 for slots 0-7, dims 10-17 for slots 8-15); its chosen key p has
+K[p, h, needle_dim(g)] = 64 and every other key has zeros in dims 0-17.  The needle scores
 2048 * D^-0.5 * log2(e) ~ 261 log2 units, every other key exactly 0, so every other P underflows to 0 and
 the output is V[p] bit for bit (or the exact mean of 2 or 4 tied needles).
 
@@ -32,7 +33,7 @@ LOG2E = 1.4426950408889634
 NEEDLE_Q = 32.0
 NEEDLE_K = 64.0
 V_MAX = 32            # V entries of the needle probes are integers in [-V_MAX, V_MAX]
-PROBE_DIMS = 10       # dims 0-7: needles (one per GQA slot), 8-9: ramp
+PROBE_DIMS = 18       # dims 0-7 and 10-17: needles (one per GQA slot), 8-9: ramp
 MIN_GAP = 160.0       # log2 units every probe maximum must beat the runner-up by
 RAMP_FP16_MAX = 2048  # fp16 ramp: positions must stay exact integers
 
@@ -55,9 +56,15 @@ def out_ulp(dtype: torch.dtype) -> float:
 
 
 # ------------------------------------------------------------------------------------------- probe values
+def needle_dim(g: int) -> int:
+    """The dim that carries the needle of GQA slot g (0..15); dims 8-9 belong to the ramp."""
+    assert 0 <= g < 16, "needle probes cover GQA groups of up to 16 query heads"
+    return g if g < 8 else g + 2
+
+
 def needle_query(g: int, d: int = 128) -> torch.Tensor:
     q = torch.zeros(d)
-    q[g] = NEEDLE_Q
+    q[needle_dim(g)] = NEEDLE_Q
     return q
 
 
@@ -82,7 +89,7 @@ def ramp_key_dims(positions: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
 
 def probe_keys(gen: torch.Generator, n: int, hkv: int, dtype: torch.dtype, d: int = 128,
                ramp: bool = True) -> torch.Tensor:
-    """Keys [n, hkv, d]: random in dims >= 10 (queries are zero there), dims 0-7 zero, dims 8-9 the ramp."""
+    """Keys [n, hkv, d]: random in dims >= 18 (queries are zero there), the needle dims zero, dims 8-9 the ramp."""
     k = torch.randn((n, hkv, d), generator=gen)
     k[..., :PROBE_DIMS] = 0
     if ramp and n:
@@ -91,7 +98,7 @@ def probe_keys(gen: torch.Generator, n: int, hkv: int, dtype: torch.dtype, d: in
 
 
 def plant_needle(k: torch.Tensor, pos: int, h: int, g: int) -> None:
-    k[pos, h, g] = NEEDLE_K
+    k[pos, h, needle_dim(g)] = NEEDLE_K
 
 
 def integer_values(gen: torch.Generator, n: int, hkv: int, dtype: torch.dtype, d: int = 128) -> torch.Tensor:
@@ -194,6 +201,68 @@ def assign_needles(kv_lens: Sequence[int], page_size: int, hq: int, seed: int = 
     return reqs
 
 
+# ------------------------------------------------------------------------------------------- long contexts
+def plan_positions(n: int, chunk: int, tile: int = 128) -> List[int]:
+    """Decode needle positions of a request of kv_len n under a plan of `chunk`-key chunks (keys 0..n-2 cached
+    and streamed in 128-key tiles, n-1 appended by the launch): both sides of every chunk boundary, the first
+    and the last tile of the streamed range, the last cached key and the appended one.  A few dozen positions
+    at any length (at most 16 chunks), where boundary_positions names every tile boundary."""
+    last_tile = (n - 2) // tile * tile if n >= 2 else 0
+    want = {0, 1, tile - 1, tile, last_tile - 1, last_tile, n - 2, n - 1}
+    for c in range(chunk, n, chunk):
+        want |= {c - 1, c}
+    return sorted(x for x in want if 0 <= x < n)
+
+
+def spread_positions(n: int, required: Sequence[int], slots: int, n_random: int, rnd: random.Random) -> List[int]:
+    """`slots` distinct positions below n: every required one, n_random random others, and random positions
+    for the rest; shuffled (so a position lands on an arbitrary query head and tie group)."""
+    pos = list(dict.fromkeys(required))
+    assert len(pos) + n_random <= slots <= n, (len(pos), n_random, slots, n)
+    taken = set(pos)
+    while len(pos) < slots:
+        x = rnd.randrange(n)
+        if x not in taken:
+            taken.add(x)
+            pos.append(x)
+    rnd.shuffle(pos)
+    return pos
+
+
+def assign_plan_needles(lens: Sequence[int], chunk: int, hq: int, seed: int = 0, ties: int = 4,
+                        n_random: int = 8) -> List[Tuple[int, List[List[int]]]]:
+    """Needles of decode requests of kv_len `lens` under a plan of `chunk`-key chunks: [(kv_len, [tied positions
+    per query head])] in the order of lens.  The requests of one length share out plan_positions(n, chunk),
+    n_random random positions and random fill, `ties` distinct positions per query head (one where the length
+    is shorter than the requests' slots; positions then repeat across heads)."""
+    rnd = random.Random(seed)
+    groups = {}
+    for n in sorted(set(lens)):
+        copies = lens.count(n)
+        t = ties if n >= copies * hq * ties else 1
+        slots = copies * hq * t
+        required = plan_positions(n, chunk)
+        assert len(required) <= slots, f"kv_len {n}: {len(required)} plan positions for {slots} needles"
+        if slots <= n:
+            pos = spread_positions(n, required, slots, min(n_random, slots - len(required)), rnd)
+        else:
+            pos = required + [rnd.randrange(n) for _ in range(slots - len(required))]
+            rnd.shuffle(pos)
+        groups[n] = [[pos[(c * hq + h) * t : (c * hq + h + 1) * t] for h in range(hq)] for c in range(copies)]
+    return [(n, groups[n].pop(0)) for n in lens]
+
+
+def sampled_rows(q_len: int, rnd: random.Random, n_random: int = 64, tile: int = 128) -> List[int]:
+    """Query rows of a long extend to check against the fp64 reference: rows 0, 1, 127, 128 and 129, both sides
+    of every 128-row query tile edge in the first and the last query tile, the last 130 rows and n_random
+    random rows."""
+    last = (q_len - 1) // tile * tile
+    want = {0, 1, tile - 1, tile, tile + 1, last - 1, last, last + 1, q_len - 1}
+    want |= set(range(max(0, q_len - 130), q_len))
+    want |= {rnd.randrange(q_len) for _ in range(n_random)}
+    return sorted(x for x in want if 0 <= x < q_len)
+
+
 # ------------------------------------------------------------------------------------------- adversarial regimes
 REGIMES = ["temp0", "temp0.25", "temp1", "temp4", "temp16", "drift_up", "drift_down", "chunk_maxima", "magnitude"]
 CHUNK_OFFSETS = [0.0, 40.0, -40.0, -135.0, 40.0, -20.0, 10.0, -60.0]  # log2 units per block of keys
@@ -208,20 +277,21 @@ def regime_request(name: str, gen: torch.Generator, n: int, n_q: int, hq: int, h
     the maximum (its merge weight underflows) and two blocks tied at it, large V (bf16 200 + N(0, 1), fp16
     +-2e4)."""
     temp = float(name[4:]) if name.startswith("temp") else 1.0
-    q = torch.randn((n_q, hq, d), generator=gen) * temp
-    k = torch.randn((n, hkv, d), generator=gen)
-    v = torch.randn((n, hkv, d), generator=gen)
-    j = torch.arange(n, dtype=torch.float64)
+    dev = gen.device  # the tensors are made where the generator lives (a CUDA generator: long contexts)
+    q = torch.randn((n_q, hq, d), generator=gen, device=dev) * temp
+    k = torch.randn((n, hkv, d), generator=gen, device=dev)
+    v = torch.randn((n, hkv, d), generator=gen, device=dev)
+    j = torch.arange(n, dtype=torch.float64, device=dev)
     off = None  # per-key score offset in log2 units, carried by dim 0 (q[0] = 16)
     if name == "drift_up":
         off = j * (8.0 / 128)
     elif name == "drift_down":
         off = (n - 1 - j) * (8.0 / 128)
     elif name == "chunk_maxima":
-        off = torch.tensor([CHUNK_OFFSETS[int(x) // block % len(CHUNK_OFFSETS)] for x in j], dtype=torch.float64)
+        off = torch.tensor(CHUNK_OFFSETS, dtype=torch.float64, device=dev)[(j.long() // block) % len(CHUNK_OFFSETS)]
     if off is not None:
         q[..., 0] = 16.0
         k[..., 0] = (off * math.log(2.0) * math.sqrt(d) / 16.0).float()[:, None]
     if name == "magnitude":
-        v = 200.0 + v if dtype == torch.bfloat16 else 2e4 * (2 * torch.rand((n, hkv, d), generator=gen) - 1)
+        v = 200.0 + v if dtype == torch.bfloat16 else 2e4 * (2 * torch.rand((n, hkv, d), generator=gen, device=dev) - 1)
     return q.to(dtype), k.to(dtype), v.to(dtype)

@@ -4,6 +4,7 @@ from __future__ import annotations
 
 import contextlib
 import importlib
+import math
 import random
 from dataclasses import dataclass
 from types import SimpleNamespace
@@ -37,6 +38,12 @@ def options(b200, **opts):
 
 # options(b200, **SPLIT_PLAN): every decode request split into 128-key chunks, as many as the plan allows
 SPLIT_PLAN = {"decode_plan_nosplit": 0, "decode_plan_target": 16}
+
+
+def table_align(page_size: int) -> int:
+    """Page-table width granule: a multiple of 64 columns and of the page size (the allocator writes whole pages;
+    24, 48 and 96 do not divide 64)."""
+    return math.lcm(64, page_size)
 
 
 @dataclass
@@ -73,7 +80,7 @@ def make_world(
     shuffle_pages: bool = True,
 ) -> World:
     g = torch.Generator().manual_seed(seed)
-    al = max(64, page_size)
+    al = table_align(page_size)
     max_seq_al = (max_seq + al - 1) // al * al  # whole pages are written by the allocator
     if num_pages is None:
         num_pages = (max_reqs * max_seq_al) // page_size + 8
@@ -174,6 +181,60 @@ def assert_bits_equal(a: torch.Tensor, b: torch.Tensor, what: str):
     assert a.shape == b.shape, f"{what}: shapes {tuple(a.shape)} vs {tuple(b.shape)}"
     assert torch.equal(a.view(torch.int16), b.view(torch.int16)), \
         f"{what}: bits differ, max |a - b| {(a.float() - b.float()).abs().max().item():.3e}"
+
+
+ORDER_CLAMP_TILES = 127  # metadata.cu kOrderBins - 1: the decode plan's counting sort puts bigger items in one bin
+PREFILL_CLAMP_TILES = 1023  # metadata.cu kPrefillBins - 1, the same for the prefill plan
+
+
+def check_decode_plan(plan: np.ndarray, kv_lens: Sequence[int], max_splits: int = 16) -> None:
+    """The split-KV decode plan {chunk, total, bs, 0, chunk_start[bs + 1], order[total]} of requests with
+    kv_lens: every (request, chunk) item exactly once, chunk_start the running chunk count, and the work order
+    descending in min(tiles, 127), tiles = the item's 128-key tiles (its last chunk without the appended key).
+    The counting sort has 128 bins, so items of 127 tiles or more (kv_len >= 16 256 unsplit) share the last bin
+    and come out in arbitrary order among themselves: a balance question, not a correctness one."""
+    kv_lens = np.asarray(kv_lens, dtype=np.int64)
+    bs = len(kv_lens)
+    chunk, total, pbs = int(plan[0]), int(plan[1]), int(plan[2])
+    assert pbs == bs and chunk % 128 == 0 and chunk >= 128
+    starts = plan[4 : 4 + bs + 1]
+    n_chunks = -(-kv_lens // chunk)
+    assert np.array_equal(np.diff(starts), n_chunks) and starts[0] == 0 and starts[-1] == total
+    assert n_chunks.max() <= max_splits
+    order = plan[4 + bs + 1 : 4 + bs + 1 + total]
+    items = [(int(e) & 0xFFFF, (int(e) >> 16) & 0xF) for e in order]
+    assert len(set(items)) == total and set(items) == {(r, c) for r in range(bs) for c in range(int(n_chunks[r]))}
+    assert all(((int(e) >> 20) & 0x1F) == n_chunks[int(e) & 0xFFFF] for e in order)
+
+    def tiles(r, c):
+        ln = min(chunk, int(kv_lens[r]) - c * chunk) - (1 if c == n_chunks[r] - 1 else 0)
+        return min(-(-ln // 128), ORDER_CLAMP_TILES)
+
+    sizes = [tiles(r, c) for r, c in items]
+    assert sizes == sorted(sizes, reverse=True), "decode work order is not descending in min(tiles, 127)"
+
+
+def check_prefill_plan(plan: np.ndarray, reqs: Sequence[Tuple[int, int, int]], request_major: bool) -> None:
+    """The prefill plan {n_items, 0, 0, 0, item[n_items]} (item = r | q_tile << 16) of reqs (table_idx, cached,
+    kv_len): one item per (request, 128-row query tile), each exactly once; size-sorted: descending in the
+    tile's K/V tiles under the causal mask, min(ceil(kv_hi / 128), 1023); request-major: requests in batch order,
+    the query tiles of a request adjacent, last tile first."""
+    q_tiles = [-(-(d - c) // 128) for (_, c, d) in reqs]
+    n = int(plan[0])
+    assert n == sum(q_tiles), (n, sum(q_tiles))
+    items = [(int(e) & 0xFFFF, (int(e) >> 16) & 0xFFFF) for e in plan[4 : 4 + n]]
+    assert len(set(items)) == n and set(items) == {(r, t) for r, nq in enumerate(q_tiles) for t in range(nq)}
+    if request_major:
+        assert items == [(r, t) for r, nq in enumerate(q_tiles) for t in reversed(range(nq))]
+        return
+
+    def work(r, t):
+        _, c, d = reqs[r]
+        kv_hi = min(d, c + min(d - c, (t + 1) * 128))
+        return min(-(-kv_hi // 128), PREFILL_CLAMP_TILES)
+
+    sizes = [work(r, t) for r, t in items]
+    assert sizes == sorted(sizes, reverse=True), "prefill work order is not descending in min(kv tiles, 1023)"
 
 
 def box_rows(page_size: int) -> int:

@@ -115,7 +115,7 @@ def exact(got, want):
 @pytest.mark.parametrize("dtype", DTYPES, ids=["bf16", "fp16"])
 def test_needle_arithmetic_is_exact(dtype):
     n = 2048
-    for g in range(8):
+    for g in range(16):  # every slot of a GQA group of up to 16 query heads
         q, k, v, _ = decode_needles(n, [777], dtype, g=g)
         s = P.scores_fp32(q[0], k)
         assert s[777].item() == float(torch.tensor(2048.0) * SL2)  # q, k exact in dtype; one product

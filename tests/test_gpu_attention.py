@@ -6,8 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import (GpuWorld, add_requests, assert_bits_equal, attn_tolerance_ok, make_inputs, make_world, options,
-                     oracle_forward, padded_reqs, poison_unowned, replan, run_attention)
+from helpers import (GpuWorld, add_requests, assert_bits_equal, attn_tolerance_ok, check_decode_plan, make_inputs,
+                     make_world, options, oracle_forward, padded_reqs, poison_unowned, replan, run_attention)
 from oracle import metadata as o_meta
 
 pytestmark = pytest.mark.gpu
@@ -36,26 +36,7 @@ def _check_metadata(md, ref: o_meta.RefMetadata, page_size: int):
     assert np.array_equal(md.flat_indices().cpu().numpy(), ref.indices_flat)
     assert np.array_equal(md.paged_page_table(page_size).cpu().numpy(), ref.page_table_paged)
     assert np.array_equal(md.get_last_indices(bs).cpu().numpy(), ref.last_indices)
-    plan = md.decode_plan.cpu().numpy()
-    chunk, total, pbs = int(plan[0]), int(plan[1]), int(plan[2])
-    assert pbs == bs and chunk % 128 == 0 and chunk >= 128
-    starts = plan[4 : 4 + bs + 1]
-    n_chunks = -(-ref.cache_seqlens // chunk)
-    assert np.array_equal(np.diff(starts), n_chunks) and starts[0] == 0 and starts[-1] == total
-    assert n_chunks.max() <= 16
-    # work order: every (request, chunk) exactly once, largest (in 128-token tiles) first
-    order = plan[4 + bs + 1 : 4 + bs + 1 + total]
-    items = {(int(e) & 0xFFFF, (int(e) >> 16) & 0xF) for e in order}
-    assert items == {(r, c) for r in range(bs) for c in range(int(n_chunks[r]))}
-    assert all(((int(e) >> 20) & 0x1F) == n_chunks[int(e) & 0xFFFF] for e in order)
-
-    def tiles(e):
-        r, c = int(e) & 0xFFFF, (int(e) >> 16) & 0xF
-        ln = min(chunk, int(ref.cache_seqlens[r]) - c * chunk) - (1 if c == n_chunks[r] - 1 else 0)
-        return -(-ln // 128)
-
-    sizes = [tiles(e) for e in order]
-    assert sizes == sorted(sizes, reverse=True)
+    check_decode_plan(md.decode_plan.cpu().numpy(), ref.cache_seqlens)
 
 
 def _run_case(b200, *, page_size, hq, hkv, lens, phase, seed=0, share_prefix=None, pad_to=None,

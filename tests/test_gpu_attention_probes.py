@@ -14,7 +14,7 @@ import pytest
 import torch
 
 from helpers import (SPLIT_PLAN, GpuWorld, World, add_requests, assert_bits_equal, options, replan, run_attention,
-                     tail_range_ends)
+                     table_align, tail_range_ends)
 from oracle import metadata as o_meta
 from oracle import probes as P
 
@@ -43,7 +43,8 @@ def _world(*, page_size, hq, hkv, dtype, lens, num_pages=None, top=False, seed=0
     the pool, starting with the last page before the dummy page."""
     need = sum(-(-d // page_size) for _, d in lens)
     num_pages = num_pages or need + 8
-    max_seq = -(-(max(d for _, d in lens) + 8) // max(64, page_size)) * max(64, page_size)
+    al = table_align(page_size)
+    max_seq = -(-(max(d for _, d in lens) + 8) // al) * al
     table = np.zeros((len(lens) + 1, max_seq), dtype=np.int32)
     table[-1, :] = num_pages * page_size
     if top:
