@@ -64,6 +64,25 @@ B200_API int b200_device_supported(void);
  * does not contain. */
 B200_API int b200_set_option(const char* name, int value);
 
+/* Event trace of the two wgmma attention kernels (decode, prefill).  With a device buffer registered, every
+ * attention launch runs an instrumented instantiation of its kernel in which lane 0 of each warp records
+ * timestamped events ({u64 %globaltimer ns, u32 %clock, u8 code, u8 warp, u16 arg}, 16 bytes) into its own
+ * region of the buffer; outputs, K/V appends and the number of launches are the same as untraced.  Layout of a
+ * region: a 64-byte header, u32 counts[grid][warps] (16-byte padded), records[grid][warps][events_per_warp]
+ * (csrc/attn.cuh; decoded by mini-sglang_b200/trace.py).  A warp that has more events than events_per_warp only
+ * counts the rest, so its count exceeds events_per_warp.
+ *   b200_attn_trace_set: buf (device, 16-byte aligned, ZERO-FILLED, at least one decode region) and
+ *     events_per_warp > 0 register the buffer and reset the counts; buf = NULL turns tracing off (the buffer is
+ *     not touched again; the counts stay readable).  Regions are handed out in launch order; once the next one
+ *     does not fit, launches run the uninstrumented kernel and are counted as untraced -- a call never fails
+ *     because of tracing.  A launch captured into a CUDA graph keeps the region it was given at capture: every
+ *     replay rewrites that region.
+ *   b200_attn_trace_launch_bytes: bytes of one region; phase 0 = decode, 1 = prefill; 0 for bad arguments.
+ *   b200_attn_trace_launches: launches given a region, launches that ran untraced because the buffer was full. */
+B200_API int b200_attn_trace_set(void* buf, size_t bytes, int events_per_warp);
+B200_API size_t b200_attn_trace_launch_bytes(int phase, int events_per_warp);
+B200_API int b200_attn_trace_launches(uint64_t* traced, uint64_t* untraced);
+
 /* ---------------------------------------------------------------------------------------
  * K1  KV append.  Replaces `store_cache(k_cache, v_cache, indices, k, v)`
  *     (M/kernel/store.py:30-42 -> M/kernel/csrc/jit/store.cu:28-53,59-121), called from

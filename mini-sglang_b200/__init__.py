@@ -6,6 +6,7 @@ Holds only what the attention hot path needs (SURVEY.md section 8):
 * ``_cabi``       ctypes binding (fails loudly if the library is missing; no CPU fallback)
 * ``ops``         operator-level host API (store_cache, rmsnorm, fused_add_rmsnorm, rope, ...)
 * ``attention``   ``B200AttnBackend`` behind the reference's ``BaseAttnBackend`` interface
+* ``trace``       event timelines recorded inside the decode / prefill attention launches
 * ``distributed`` one-shot NVLink all-reduce behind the reference's ``DistributedCommunicator`` plug-in point
 * ``kvcache`` / ``layers`` / ``core`` / ``utils``  interface mirrors of the reference types the
   boundary touches, for use where the reference is not installed
@@ -14,7 +15,7 @@ The directory name is not a Python identifier: import it with
 ``importlib.import_module("mini-sglang_b200")`` or through the ``minisgl_b200`` shim package.
 """
 
-from . import _cabi, attention, core, distributed, kvcache, layers, ops, utils  # noqa: F401
+from . import _cabi, attention, core, distributed, kvcache, layers, ops, trace, utils  # noqa: F401
 from .attention import (  # noqa: F401
     BACKEND_NAME,
     SUPPORTED_ATTENTION_BACKENDS,
@@ -24,8 +25,10 @@ from .attention.backend import B200AttnBackend, B200Metadata  # noqa: F401
 from .build import build as build_native  # noqa: F401
 from .core import Batch, Context, Req, get_global_ctx, set_global_ctx  # noqa: F401
 from .kvcache import MHAKVCache  # noqa: F401
+from .trace import AttentionTrace, summarise, to_chrome_trace  # noqa: F401
 
 __all__ = [
+    "AttentionTrace",
     "B200AttnBackend",
     "B200Metadata",
     "BACKEND_NAME",
@@ -44,5 +47,8 @@ __all__ = [
     "layers",
     "ops",
     "set_global_ctx",
+    "summarise",
+    "to_chrome_trace",
+    "trace",
     "utils",
 ]

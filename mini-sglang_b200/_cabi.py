@@ -14,7 +14,7 @@ from typing import Optional
 _LIB: Optional[C.CDLL] = None
 LIB_PATH = Path(__file__).resolve().parent / "libb200attn.so"
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 _i32, _i64, _f32, _vp, _sz = C.c_int, C.c_int64, C.c_float, C.c_void_p, C.c_size_t
 
@@ -63,6 +63,9 @@ SIGNATURES = {
         [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _vp]
         + [_i32, _i64, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _sz, _i32, _vp],
     ),
+    "b200_attn_trace_set": (_i32, [_vp, _sz, _i32]),
+    "b200_attn_trace_launch_bytes": (_sz, [_i32, _i32]),
+    "b200_attn_trace_launches": (_i32, [C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "b200_ar_region_bytes": (_sz, [_i32, _sz]),
     "b200_ar_alloc": (_i32, [_sz, C.POINTER(_vp)]),
     "b200_ar_ipc_handle": (_i32, [_vp, _vp]),

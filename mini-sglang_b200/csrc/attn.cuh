@@ -170,4 +170,126 @@ __device__ __forceinline__ void tma_load_group(uint32_t dst, const CUtensorMap* 
   sm90::tma_load_2d(dst + 384, m, bar, col, rows.w);
 }
 
+// ------------------------------------------------------------------------------ event trace
+// b200_attn_trace_set registers a device buffer; each traced launch gets one region of it (mini-sglang_b200/trace.py
+// decodes the same layout):
+//   TraceHeader (64 B) | u32 count[grid][warps], rounded up to 16 B | TraceRecord rec[grid][warps][events_per_warp]
+// Lane 0 of every warp records the events of its warp with plain stores; past events_per_warp it only counts, and
+// writes the count (which then exceeds events_per_warp) when the CTA ends.  Only the kTrace = true instantiations of
+// the two wgmma kernels contain any of it.
+constexpr uint32_t kTraceMagic = 0x52545441u;  // "ATTR"
+constexpr uint32_t kTraceVersion = 1;
+constexpr int kTracePhaseDecode = 0, kTracePhasePrefill = 1;
+constexpr int kDecodeWarps = 10, kPrefillWarps = 12;
+enum TraceFlag : uint32_t { kTraceFused = 1, kTraceInKernelCombine = 2, kTraceEarlyKv = 4 };
+
+// Event codes; arg is %smid, the unit's position k in the CTA's list, or the tile's index within its unit.
+enum TraceCode : uint32_t {
+  kEvBegin = 1,        // first event of every warp, arg = %smid
+  kEvPdlWait = 2,      // past griddepcontrol.wait
+  kEvUnitBegin = 3,    // arg = k (every unit of the CTA's list, in every role, also those the role skips)
+  kEvUnitEnd = 4,      // arg = k
+  kEvEmptyWait = 5,    // producer: waits for a free ring slot, arg = tile
+  kEvEmptyDone = 6,    // producer: the slot is free, arg = tile
+  kEvIssued = 7,       // producer: the tile's loads are issued, arg = tile
+  kEvQIssued = 8,      // prefill K producer: the unit's Q tile load is issued, arg = k
+  kEvAppend = 9,       // prefill producers: the append stores of a tile are issued, arg = tile
+  kEvQReady = 10,      // decode Q loader: operand (and fused epilogue rows) written; consumer: Q operand landed
+  kEvKFull = 11,       // consumer: K tile landed, arg = tile
+  kEvQK = 12,          // consumer: S = QK^T complete
+  kEvSoftmax = 13,     // consumer: P written / in registers
+  kEvVFull = 14,       // consumer: V tile landed
+  kEvPV = 15,          // consumer: O += PV complete
+  kEvSkip = 16,        // prefill consumer: tile fully masked for the warpgroup, no MMA
+  kEvEpiBegin = 17,    // consumer epilogue (decode: new-token score, append, output or partial store), arg = k
+  kEvEpiEnd = 18,
+  kEvArrive = 19,      // decode combiner: counted in, another chunk merges, arg = k
+  kEvArriveLast = 20,  // decode combiner: counted in last, merges, arg = k
+  kEvMergeBegin = 21,
+  kEvMergeEnd = 22,
+  kEvEnd = 31,         // last event of every warp: past the kernel's final __syncthreads
+};
+
+struct TraceHeader {
+  uint32_t magic, version, phase, grid, threads, warps, bs, hq, hkv, group, page_size, box_rows, events_per_warp,
+      plan_kind, seq, flags;
+};
+static_assert(sizeof(TraceHeader) == 64, "trace header is 64 bytes");
+struct TraceRecord {  // 16 bytes, one st.global.v4
+  uint64_t globaltimer_ns;
+  uint32_t clock;
+  uint8_t code, warp;
+  uint16_t arg;
+};
+static_assert(sizeof(TraceRecord) == 16, "trace record is 16 bytes");
+
+__host__ __device__ inline size_t trace_counts_bytes(int grid, int warps) { return ((size_t)grid * warps * 4 + 15) / 16 * 16; }
+inline size_t trace_region_bytes(int grid, int warps, int events_per_warp) {
+  return sizeof(TraceHeader) + trace_counts_bytes(grid, warps) + (size_t)grid * warps * events_per_warp * sizeof(TraceRecord);
+}
+
+// What a traced launch is handed: its region (nullptr = not traced), the record capacity, its sequence number, and
+// header fields the kernel does not know.  The header's plan_kind is 1 for a decode plan that splits, else 0.
+struct TraceArgs {
+  uint8_t* region;
+  int events_per_warp, seq, page_size;
+  uint32_t flags;
+};
+// capi.cu: the next region for a launch of `phase` with `grid` CTAs; false (and counted as untraced) when no buffer
+// is registered or the regions are used up.
+bool trace_next_region(int phase, int grid, TraceArgs* out);
+
+// One warp's event writer, kWarps warps per CTA: WarpTrace<false, .> is empty and compiles to nothing.  The traced
+// state is three registers (lane 0's record pointer, nullptr in the other lanes, and the event count); everything
+// else is read from the kernel parameters when needed, so the producer warps' small register budget holds it.
+template <bool kOn, int kWarps>
+struct WarpTrace {
+  __device__ __forceinline__ explicit WarpTrace(const TraceArgs&) {}
+  __device__ __forceinline__ void ev(uint32_t, int) {}
+  __device__ __forceinline__ void begin() {}
+  __device__ __forceinline__ void header(int, int, int, int, int, int) {}
+  __device__ __forceinline__ void finish() {}
+};
+template <int kWarps>
+struct WarpTrace<true, kWarps> {
+  const TraceArgs& t;
+  TraceRecord* rec;
+  uint32_t n;
+  __device__ __forceinline__ static size_t slot() { return (size_t)blockIdx.x * kWarps + threadIdx.x / kWarp; }
+  __device__ __forceinline__ explicit WarpTrace(const TraceArgs& args) : t(args), rec(nullptr), n(0) {
+    if (threadIdx.x % kWarp == 0)
+      rec = reinterpret_cast<TraceRecord*>(t.region + sizeof(TraceHeader) + trace_counts_bytes(gridDim.x, kWarps)) +
+            slot() * t.events_per_warp;
+  }
+  __device__ __forceinline__ void ev(uint32_t code, int arg) {
+    if (rec == nullptr) return;
+    if (n < (uint32_t)t.events_per_warp) {
+      uint64_t ns;
+      uint32_t clk;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
+      asm volatile("mov.u32 %0, %%clock;" : "=r"(clk));
+      const uint32_t tag = code | ((threadIdx.x / kWarp) << 8) | ((uint32_t)arg << 16);
+      asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(rec + n), "r"((uint32_t)ns),
+                   "r"((uint32_t)(ns >> 32)), "r"(clk), "r"(tag));
+    }
+    ++n;
+  }
+  __device__ __forceinline__ void begin() {
+    uint32_t sm;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    ev(kEvBegin, (int)sm);
+  }
+  // CTA 0, warp 0: the launch's header
+  __device__ __forceinline__ void header(int phase, int bs, int hq, int hkv, int box_rows, int plan_kind) {
+    if (rec == nullptr || blockIdx.x != 0 || threadIdx.x != 0) return;
+    *reinterpret_cast<TraceHeader*>(t.region) =
+        TraceHeader{kTraceMagic, kTraceVersion, (uint32_t)phase, gridDim.x, blockDim.x, (uint32_t)kWarps,
+                    (uint32_t)bs, (uint32_t)hq, (uint32_t)hkv, (uint32_t)(hq / hkv), (uint32_t)t.page_size,
+                    (uint32_t)box_rows, (uint32_t)t.events_per_warp, (uint32_t)plan_kind, (uint32_t)t.seq, t.flags};
+  }
+  __device__ __forceinline__ void finish() {
+    if (rec != nullptr) reinterpret_cast<uint32_t*>(t.region + sizeof(TraceHeader))[slot()] = n;
+  }
+};
+
 }  // namespace b200

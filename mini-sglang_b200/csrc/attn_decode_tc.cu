@@ -118,6 +118,7 @@ struct Params {
   float eps;
   const int32_t* positions;
   const float* cos_sin;  // fp32 [max_pos][128] = cos | sin
+  TraceArgs trace;       // read by the kTrace = true instantiation only
 };
 
 struct Unit {
@@ -155,7 +156,8 @@ __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_
     wgmma_m64n16k16_ss<kTransA>(d, da, db, scale_d, tsel);
 }
 
-template <typename T, int G>
+// kTrace: each warp records its events into p.trace (attn.cuh); the false instantiation is the product kernel.
+template <typename T, int G, bool kTrace>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map_k,
                       const __grid_constant__ CUtensorMap map_v,
@@ -173,6 +175,8 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   const int tid = threadIdx.x, warp = tid / kWarp, lane = tid % kWarp;
   auto bar = [&](int i) { return sbase + Smem::bars + i * 8; };
   float* red = reinterpret_cast<float*>(smem + Smem::red);
+  WarpTrace<kTrace, kDecodeWarps> tr(p.trace);
+  tr.begin();
 
   // ---------------------------------------------------------------- setup that touches no global memory
   // zero the Q operand buffers whose padding rows (heads >= G) are never written again
@@ -216,7 +220,9 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   //    predecessor's tail (or a small kernel in between, e.g. the TP all-reduce) overlap.
   if (!p.early) pdl_wait();
   pdl_launch_dependents();
+  if (!p.early) tr.ev(kEvPdlWait, 0);
   const int chunk_tokens = p.plan[0];
+  tr.header(kTracePhaseDecode, p.bs, p.hq, p.hkv, p.box_rows, p.plan[1] != p.bs);
   const int32_t* order = p.plan + kPlanHeader + p.bs + 1;
   const auto units = deal_units<Unit, kUnitSlotBytes, kMaxUnitsSmem>(
       smem + Smem::units, p.plan[1] * p.hkv,
@@ -243,7 +249,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       RingCursor<kStages> kv;
       for (int k = 0; k < units.n_rounds; ++k) {
         const Unit u = units.at(k);
-        if (u.n_tiles <= 0) continue;
+        if constexpr (kTrace)
+          if (!units.none(u)) tr.ev(kEvUnitBegin, k);
+        if (u.n_tiles <= 0) {
+          if constexpr (kTrace)
+            if (!units.none(u)) tr.ev(kEvUnitEnd, k);
+          continue;
+        }
         const int32_t* slots = p.slot_table + (int64_t)u.r * p.st_stride;
         const int col0 = u.h * kD;
         if (rb == 0) {
@@ -256,10 +268,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           for (int t = 0; t < u.n_tiles; ++t, kv.advance()) {
             const int4 cur = nxt;
             if (t + 1 < u.n_tiles) nxt = load_group(t + 1);
+            tr.ev(kEvEmptyWait, t);
             kv.wait_empty(bar(empty0));
+            tr.ev(kEvEmptyDone, t);
             if ((warp & 1) == 0 && lane == 0) mbar_arrive_expect_tx(bar(full0 + kv.stage()), kKvTileBytes);
             __syncwarp();
             tma_load_group(L.dst(ring, kv.stage()), gmap, bar(full0 + kv.stage()), L.col(col0), cur);
+            tr.ev(kEvIssued, t);
           }
         } else {
           // ---- box mode
@@ -282,7 +297,9 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             if (lane < n_instr && left > 0) first_slot = __ldg(slots + pb);
             // the stage's transaction bytes are exactly the rows the lanes issue below
             const uint32_t tx_bytes = __reduce_add_sync(0xffffffffu, (uint32_t)rows) * 128u;
+            tr.ev(kEvEmptyWait, t);
             kv.wait_empty(bar(empty0));
+            tr.ev(kEvEmptyDone, t);
             const uint32_t fb = bar(full0 + kv.stage());
             if (lane == 0) mbar_arrive_expect_tx(fb, tx_bytes);
             __syncwarp();
@@ -296,21 +313,30 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
                 for (int r = 0; r < rows; r += 8) tma_load_2d(dst + r * 128, tmap, fb, col, first_slot + r);
               }
             }
+            tr.ev(kEvIssued, t);
           }
         }
+        tr.ev(kEvUnitEnd, k);
       }
     }
   } else if (warp == kWarpQ) {
     // ============================================================ Q loader
-    if (p.early) pdl_wait();
+    if (p.early) {
+      pdl_wait();
+      tr.ev(kEvPdlWait, 0);
+    }
     RingCursor<2> qr;
     RingCursor<Smem::kEpiSlots> er;
     for (int k = 0; k < units.n_rounds; ++k) {
       const Unit u = units.at(k);
       if (units.none(u)) continue;
+      tr.ev(kEvUnitBegin, k);
       const bool need_q = u.n_tiles > 0;                 // the tensor core needs the Q operand
       const bool need_epi = p.fuse && u.last_chunk;      // the epilogue needs roped q / k rows
-      if (!need_q && !need_epi) continue;
+      if (!need_q && !need_epi) {
+        tr.ev(kEvUnitEnd, k);
+        continue;
+      }
       const uint32_t qb = qr.stage(), es = er.stage();
       if (need_q) qr.wait_empty(bar(kQEmpty));
       if (need_epi) er.wait_empty(bar(kEpiEmpty));
@@ -349,12 +375,17 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
         if (need_q) mbar_arrive(bar(kQFull + qb));
         if (need_epi) mbar_arrive(bar(kEpiFull + es));
       }
+      tr.ev(kEvQReady, k);
       if (need_q) qr.advance();
       if (need_epi) er.advance();
+      tr.ev(kEvUnitEnd, k);
     }
   } else if (warp >= 4 && warp < 8) {
     // ============================================================ consumer warpgroup (128 threads)
-    if (p.early) pdl_wait();
+    if (p.early) {
+      pdl_wait();
+      tr.ev(kEvPdlWait, 0);
+    }
     constexpr bool kTransV = true;  // A = V^T: the head dims (M) are the contiguous axis of a V tile
     T* const tsel = nullptr;        // selects the bf16 / fp16 wgmma overload
     const int ct = tid - 128;       // 0..127
@@ -377,6 +408,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     for (int k = 0; k < units.n_rounds; ++k) {
       const Unit u = units.at(k);
       if (units.none(u)) continue;
+      tr.ev(kEvUnitBegin, k);
       float acc[2][N / 2], l_thr[kE], m_run[kE];
 #pragma unroll
       for (int e = 0; e < kE; ++e) {
@@ -422,11 +454,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       if (u.n_tiles > 0) {
         const uint32_t qb = qr.stage();
         qr.wait_full(bar(kQFull));
+        tr.ev(kEvQReady, k);
         const uint32_t qa = sbase + Smem::qbuf + qb * Smem::kQBufBytes;
         for (int j = 0; j < u.n_tiles; ++j, kv.advance()) {
           const uint32_t stage = kv.stage();
           // ---- S^T = K_tile . Q^T: A = K rows (K-major, 128B swizzle), B = Q rows (K-major, 8-row atoms 1024 B apart)
           kv.wait_full(bar(kFullK));
+          tr.ev(kEvKFull, j);
           const uint32_t kb = sbase + Smem::kring + stage * kKvTileBytes;
           float s[2][N / 2];
 #pragma unroll
@@ -444,6 +478,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             }
           wgmma_commit();
           wgmma_wait0();
+          tr.ev(kEvQK, j);
           __syncwarp();
           if (lane == 0) {
             mbar_arrive(bar(kEmptyK + stage));                      // the K tile is dead
@@ -514,8 +549,10 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           for (int e = 0; e < kE; ++e) l_thr[e] = l_thr[e] * alpha[e] + psum[e];
           fence_proxy_async_smem();  // P^T (and zeroed V rows) visible to the tensor core
           named_bar_sync(1, 128);    // every warp's P^T is written; the tile maxima may be overwritten
+          tr.ev(kEvSoftmax, j);
           // ---- O^T += V_tile^T . P^T: A = V rows read MN-major, B = P^T (K-major, no swizzle)
           kv.wait_full(bar(kFullV));
+          tr.ev(kEvVFull, j);
           const uint32_t vb = sbase + Smem::vring + stage * kKvTileBytes;
           const uint32_t pb = sbase + Smem::pbuf;
           wgmma_fence();
@@ -531,11 +568,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             }
           wgmma_commit();
           wgmma_wait0();
+          tr.ev(kEvPV, j);
           __syncwarp();
           if (lane == 0) mbar_arrive(bar(kEmptyV + stage));
         }
         qr.advance();
       }
+      tr.ev(kEvEpiBegin, k);
 
       // ---- unit epilogue on CUDA cores: row sums, the appended token (score, value, pool append), output.
       // Reduction scratch double buffered by unit parity: the next unit may write its slots while
@@ -617,6 +656,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
             if (col_of(slot_of(i)) < G)
               p.out[((int64_t)u.r * p.hq + u.h * G + h0 + (i & 1) + (i >> 2) * 8) * kD + row_of(mb, i)] =
                   DTypeTraits<T>::from_float(acc[mb][i] * inv[slot_of(i)]);
+        tr.ev(kEvEpiEnd, k);
       } else {
         const int64_t base = ((int64_t)u.r * kMaxSplits + u.c) * p.hq + u.h * G;
 #pragma unroll
@@ -633,6 +673,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
               p.part_ml[(base + h0 + (e & 1) + (e >> 1) * 8) * 2 + 1] = l_tot[e];
             }
         }
+        tr.ev(kEvEpiEnd, k);
         // ---- hand the unit to the combiner warp (asynchronous split-KV merge): the consumer warps
         // only pay an mbarrier arrive; the release/acquire pair orders the partial stores above
         // before the combiner's device-scope fence + arrival counter.
@@ -642,16 +683,25 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           fr.advance();
         }
       }
+      tr.ev(kEvUnitEnd, k);
     }
   } else if (warp == kWarpCombine) {
     // ============================================================ split-KV combiner (one warp)
     // For every multi-chunk unit of this CTA: count in on the (request, kv head) arrival counter;
     // whoever arrives last merges all partials (flash-decoding reduction) and writes the output.
-    if (p.early) pdl_wait();
+    if (p.early) {
+      pdl_wait();
+      tr.ev(kEvPdlWait, 0);
+    }
     if (p.fused_combine) {
       RingCursor<kFinRing> fr;
       for (int k = 0; k < units.n_rounds; ++k) {
         const Unit u = units.at(k);
+        if constexpr (kTrace)
+          if (!units.none(u)) {
+            tr.ev(kEvUnitBegin, k);
+            if (u.n_chunks == 1) tr.ev(kEvUnitEnd, k);
+          }
         if (units.none(u) || u.n_chunks == 1) continue;
         const uint32_t slot = fr.stage();
         fr.wait_full(bar(kFinFull));
@@ -664,7 +714,9 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           if (last) p.counters[u.r * p.hkv + u.h] = 0;  // zero again for the next launch
         }
         last = __shfl_sync(0xffffffffu, last, 0);
+        tr.ev(last ? kEvArriveLast : kEvArrive, k);
         if (last) {
+          tr.ev(kEvMergeBegin, k);
           __threadfence();  // acquire the other chunks' partials
           // Heads in passes of GB <= 8: (o, m, l, weight, 1/l) of 9-16 heads plus their prefetched partials would
           // not fit one warp's registers.  A group of 9-15 ends its last pass at head G-1, so that pass merges some
@@ -731,29 +783,47 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
               *reinterpret_cast<uint2*>(p.out + ((int64_t)u.r * p.hq + u.h * G + g0 + g) * kD + lane * 4) = pk;
             }
           }
+          tr.ev(kEvMergeEnd, k);
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(bar(kFinEmpty + slot));
+        tr.ev(kEvUnitEnd, k);
       }
     }
   }
 
   // ---------------------------------------------------------------- teardown
   __syncthreads();
+  tr.ev(kEvEnd, 0);
+  tr.finish();
 }
 
-template <typename T, int G>
-static int launch_g(const Params<T>& p, const CUtensorMap& mk, const CUtensorMap& mv,
-                    const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& tk,
-                    const CUtensorMap& tv, cudaStream_t st) {
+template <typename T, int G, bool kTrace>
+static int launch_kernel(const Params<T>& p, const CUtensorMap& mk, const CUtensorMap& mv, const CUtensorMap& bk,
+                         const CUtensorMap& bv, const CUtensorMap& tk, const CUtensorMap& tv, cudaStream_t st) {
   const size_t smem = Smem<kNOf<G>>::total + 1024;
   static bool configured = false;
   if (!configured) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_decode_tc_kernel<T, G>,
+    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_decode_tc_kernel<T, G, kTrace>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(attn_decode_tc_kernel<T, G>, dim3(num_sms()), dim3(kThreads), smem, st, p, mk, mv, bk, bv, tk, tv));
+  B200_CHECK_CUDA(launch_pdl(attn_decode_tc_kernel<T, G, kTrace>, dim3(num_sms()), dim3(kThreads), smem, st, p, mk, mv,
+                             bk, bv, tk, tv));
+  return 0;
+}
+
+template <typename T, int G>
+static int launch_g(Params<T> p, const CUtensorMap& mk, const CUtensorMap& mv,
+                    const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& tk,
+                    const CUtensorMap& tv, cudaStream_t st) {
+  // a registered trace buffer with a region left selects the instrumented instantiation (same launch otherwise)
+  if (trace_next_region(kTracePhaseDecode, num_sms(), &p.trace)) {
+    p.trace.flags = (p.fuse ? kTraceFused : 0u) | (p.fused_combine ? kTraceInKernelCombine : 0u) | (p.early ? kTraceEarlyKv : 0u);
+    if (int rc = launch_kernel<T, G, true>(p, mk, mv, bk, bv, tk, tv, st)) return rc;
+  } else {
+    if (int rc = launch_kernel<T, G, false>(p, mk, mv, bk, bv, tk, tv, st)) return rc;
+  }
   B200_POST_LAUNCH();
   if (!p.fused_combine) {
     B200_CHECK_CUDA(launch_pdl(attn_combine_kernel<T>, dim3(p.bs, p.hq), dim3(kHeadDim), 0, st,
@@ -780,7 +850,8 @@ static int launch(const DecodeArgs& a) {
                     (T*)a.v_cache, a.out_loc, a.slot_table, a.st_stride, a.seq_lens, a.plan, a.bs, a.hq, a.hkv,
                     (int)a.num_slots, box_rows_for(a.page_size), g_decode_exact_tail.load() ? 1 : 0, fused,
                     a.scale * kLog2e, (T*)a.out, ws.part_o, ws.part_ml, ws.counters, early, a.fuse,
-                    (const T*)a.qw, (const T*)a.kw, a.eps, a.positions, a.cos_sin};
+                    (const T*)a.qw, (const T*)a.kw, a.eps, a.positions, a.cos_sin,
+                    TraceArgs{nullptr, 0, 0, a.page_size, 0}};
   const bool bf16 = std::is_same<T, __nv_bfloat16>::value;
   CUtensorMap mk, mv;
   if (int rc = kv_pool_maps(&mk, &mv, a.k_cache, a.v_cache, a.num_slots, a.hkv, 1, bf16)) return rc;

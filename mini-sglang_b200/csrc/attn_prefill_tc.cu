@@ -65,6 +65,7 @@ struct Params {
   const int32_t* out_loc;
   int64_t nnz;
   int skip_append;  // debug: measure the attention without the fused append
+  TraceArgs trace;  // read by the kTrace = true instantiation only
 };
 
 struct Unit {
@@ -96,7 +97,8 @@ __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <typename T>
+// kTrace: each warp records its events into p.trace (attn.cuh); the false instantiation is the product kernel.
+template <typename T, bool kTrace>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map_q,
                        const __grid_constant__ CUtensorMap map_k,
@@ -112,6 +114,9 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
   const uint32_t sbase = smem_u32(smem);
   const int tid = threadIdx.x, warp = tid / kWarp, lane = tid % kWarp;
   auto bar = [&](int i) { return sbase + Smem::bars + i * 8; };
+  WarpTrace<kTrace, kPrefillWarps> tr(p.trace);
+  tr.begin();
+  tr.header(kTracePhasePrefill, p.bs, p.hq, p.hkv, p.box_rows, 0);
 
   const int group = p.hq / p.hkv;
   const int32_t* items = p.plan + 4;
@@ -173,6 +178,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     // valid: 0 = nothing, 1 = tile issued (append once it has landed), 2 = stores issued
     auto issue_stores = [&](int stage) {  // whole warp; the tile has landed
       Pending& pd = pend[stage];
+      tr.ev(kEvAppend, pd.tile_begin / kKvTileRows);
       if (rb > 0) {
         if (lane < KvLane::box_lanes(rb)) {
           const KvLane L = KvLane::box(lane, rb);
@@ -216,6 +222,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     for (int k = 0; k < units.n_rounds; ++k) {
       const Unit u = units.at(k);
       if (u.n_tiles <= 0) continue;
+      tr.ev(kEvUnitBegin, k);
       const int32_t* slots = p.slot_table + (int64_t)u.r * p.st_stride;
       const int col0 = u.h * kD;
       const bool owner = !p.skip_append && u.owner;
@@ -234,6 +241,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
                         u.q_begin + u.q_start);
         }
         __syncwarp();
+        tr.ev(kEvQIssued, k);
       };
       // Positions < cached come from the pool through the slot table; positions >= cached are the
       // tokens of this very forward and are read straight from the k / v inputs (row q_begin + pos -
@@ -260,7 +268,9 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
           const bool old_box = pb + rb <= u.cached, new_box = pb >= u.cached;
           int first_slot = p.num_slots;
           if (lane < n_instr && old_box) first_slot = __ldg(slots + pb);
+          tr.ev(kEvEmptyWait, t);
           kv.wait_empty(bar(empty0));
+          tr.ev(kEvEmptyDone, t);
           flush_stage(stage);
           if (lane == 0) mbar_arrive_expect_tx(fb, kKvTileBytes);
           __syncwarp();
@@ -273,7 +283,9 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
           }
         } else {
           // row mode: 32 row groups of four x 2 halves = 2 groups per lane, one single-row box per row
+          tr.ev(kEvEmptyWait, t);
           kv.wait_empty(bar(empty0));
+          tr.ev(kEvEmptyDone, t);
           flush_stage(stage);
           if (lane == 0) mbar_arrive_expect_tx(fb, kKvTileBytes);
           __syncwarp();
@@ -287,6 +299,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
               load_rows_one_by_one(L.dst(ring, stage), fb, L.col(col0), pos0, 4);
           }
         }
+        tr.ev(kEvIssued, t);
         if (kind == 0 && t == 0) load_q();
         // tiles issued earlier may have landed by now
         for (int s2 = 0; s2 < kStages; ++s2)
@@ -304,6 +317,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
         }
       }
       qr.advance();
+      tr.ev(kEvUnitEnd, k);
     }
     // tiles still waiting for their append: wait until they have landed, store, drain
     for (int s = 0; s < kStages; ++s)
@@ -328,6 +342,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     for (int k = 0; k < units.n_rounds; ++k) {
       const Unit u = units.at(k);
       if (u.n_tiles <= 0) continue;
+      tr.ev(kEvUnitBegin, k);
       // keys [0, vis_end) are visible to a query row; the warpgroup's last row bounds the tiles it needs
       const int vis0 = min(u.cached + u.q_start + ra + 1, u.kv_len);
       const int vis1 = min(u.cached + u.q_start + ra + 9, u.kv_len);
@@ -337,6 +352,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
       for (int i = 0; i < 64; ++i) o[i] = 0.f;
       float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
       qr.wait_full(bar(kQFull));
+      tr.ev(kEvQReady, k);
       qr.advance();
       const uint32_t qa = sbase + Smem::q + wg * 8192;  // 64 rows x 128 B into each half
       for (int j = 0; j < u.n_tiles; ++j, kv.advance()) {
@@ -344,6 +360,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
         const int tile_begin = j * kKvTileRows;
         const bool active = tile_begin < wg_vis;  // warpgroup-uniform
         kv.wait_full(bar(kFullK));
+        tr.ev(kEvKFull, j);
         float s[64];
         if (active) {
           const uint32_t kb = sbase + Smem::kring + stage * kKvTileBytes;
@@ -358,6 +375,9 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
           }
           wgmma_commit();
           wgmma_wait0();
+          tr.ev(kEvQK, j);
+        } else {
+          tr.ev(kEvSkip, j);
         }
         __syncwarp();
         if (lane == 0) {
@@ -405,8 +425,10 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
             pa[kb][2] = pack2<T>(s[8 * kb + 4], s[8 * kb + 5]);
             pa[kb][3] = pack2<T>(s[8 * kb + 6], s[8 * kb + 7]);
           }
+          tr.ev(kEvSoftmax, j);
         }
         kv.wait_full(bar(kFullV));
+        tr.ev(kEvVFull, j);
         if (active) {
           const uint32_t vb = sbase + Smem::vring + stage * kKvTileBytes;
           wgmma_fence();
@@ -418,11 +440,13 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
           }
           wgmma_commit();
           wgmma_wait0();
+          tr.ev(kEvPV, j);
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(bar(kEmptyV + stage));
       }
       // ---- epilogue: O / l -> out, rows ra and ra + 8 (row sums reduced over the quad)
+      tr.ev(kEvEpiBegin, k);
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         l_run[e] += __shfl_xor_sync(0xffffffffu, l_run[e], 1);
@@ -439,18 +463,39 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
             *reinterpret_cast<uint32_t*>(orow + 8 * i) = pack2<T>(o[4 * i + 2 * e] * inv[e], o[4 * i + 2 * e + 1] * inv[e]);
         }
       }
+      tr.ev(kEvEpiEnd, k);
+      tr.ev(kEvUnitEnd, k);
     }
   }
 
   // ---------------------------------------------------------------- teardown
   __syncthreads();
+  tr.ev(kEvEnd, 0);
+  tr.finish();
+}
+
+template <typename T, bool kTrace>
+static int launch_kernel(const Params<T>& p, cudaStream_t st, const CUtensorMap& mq, const CUtensorMap& mk,
+                         const CUtensorMap& mv, const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& nk,
+                         const CUtensorMap& nv, const CUtensorMap& nbk, const CUtensorMap& nbv) {
+  const size_t smem = Smem::total + 1024;
+  static bool configured = false;
+  if (!configured) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_tc_kernel<T, kTrace>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured = true;
+  }
+  attn_prefill_tc_kernel<T, kTrace><<<num_sms(), kThreads, smem, st>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
+  B200_POST_LAUNCH();
+  return 0;
 }
 
 template <typename T>
 static int launch(const PrefillArgs& a) {
-  const Params<T> p{a.slot_table, a.st_stride, a.seq_lens, a.cu_q, a.plan, a.bs, a.hq, a.hkv, (int)a.num_slots,
+  Params<T> p{a.slot_table, a.st_stride, a.seq_lens, a.cu_q, a.plan, a.bs, a.hq, a.hkv, (int)a.num_slots,
                     box_rows_for(a.page_size), a.scale * kLog2e, (T*)a.out, (const T*)a.k, (const T*)a.v, a.k_rs,
-                    (T*)a.k_cache, (T*)a.v_cache, a.out_loc, a.nnz, g_prefill_skip_append.load()};
+                    (T*)a.k_cache, (T*)a.v_cache, a.out_loc, a.nnz, g_prefill_skip_append.load(),
+                    TraceArgs{nullptr, 0, 0, a.page_size, 0}};
   const bool bf16 = std::is_same<T, __nv_bfloat16>::value;
   const uint64_t cols = (uint64_t)p.hkv * kD;
   CUtensorMap mq, mk, mv, nk, nv;
@@ -468,16 +513,10 @@ static int launch(const PrefillArgs& a) {
     if (int rc = encode_tensor_map_2d(&nbk, p.k_new, a.nnz, cols, p.kv_rs * 2, 64, p.box_rows, bf16)) return rc;
     if (int rc = encode_tensor_map_2d(&nbv, p.v_new, a.nnz, cols, p.kv_rs * 2, 64, p.box_rows, bf16)) return rc;
   }
-  const size_t smem = Smem::total + 1024;
-  static bool configured = false;
-  if (!configured) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_tc_kernel<T>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = true;
-  }
-  attn_prefill_tc_kernel<T><<<num_sms(), kThreads, smem, a.stream>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
-  B200_POST_LAUNCH();
-  return 0;
+  // a registered trace buffer with a region left selects the instrumented instantiation (same launch otherwise)
+  if (trace_next_region(kTracePhasePrefill, num_sms(), &p.trace))
+    return launch_kernel<T, true>(p, a.stream, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
+  return launch_kernel<T, false>(p, a.stream, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
 }
 
 }  // namespace ptc

@@ -2,10 +2,12 @@
 // accounting, device probe.  Errors follow the reference's convention of surfacing native
 // failures as Python RuntimeError (python/minisgl/kernel/csrc/include/minisgl/utils.h:40-88):
 // every entry point returns non-zero and leaves a message here.
+#include "attn.cuh"
 #include "b200attn.h"
 #include "common.cuh"
 
 #include <cstring>
+#include <mutex>
 
 namespace b200 {
 
@@ -54,7 +56,80 @@ static const struct {
 };
 }  // namespace b200
 
-extern "C" int b200_abi_version(void) { return 7; }
+// ------------------------------------------------------------------------------ event trace
+// The registered buffer is handed out front to back, one region per traced launch (attn.cuh TraceHeader).
+namespace b200 {
+static std::mutex g_trace_mu;
+static std::atomic<bool> g_trace_on{false};
+static struct {
+  uint8_t* buf = nullptr;
+  size_t bytes = 0, used = 0;
+  int events_per_warp = 0;
+  uint64_t traced = 0, untraced = 0;
+} g_trace;
+
+static int trace_warps(int phase) { return phase == kTracePhaseDecode ? kDecodeWarps : kPrefillWarps; }
+
+bool trace_next_region(int phase, int grid, TraceArgs* out) {
+  if (!g_trace_on.load(std::memory_order_relaxed)) return false;
+  std::lock_guard<std::mutex> lock(g_trace_mu);
+  if (g_trace.buf == nullptr) return false;
+  const size_t need = trace_region_bytes(grid, trace_warps(phase), g_trace.events_per_warp);
+  if (g_trace.bytes - g_trace.used < need) {
+    ++g_trace.untraced;
+    return false;
+  }
+  out->region = g_trace.buf + g_trace.used;
+  out->events_per_warp = g_trace.events_per_warp;
+  out->seq = (int)g_trace.traced;
+  g_trace.used += need;
+  ++g_trace.traced;
+  return true;
+}
+}  // namespace b200
+
+extern "C" size_t b200_attn_trace_launch_bytes(int phase, int events_per_warp) {
+  using namespace b200;
+  if ((phase != kTracePhaseDecode && phase != kTracePhasePrefill) || events_per_warp <= 0) return 0;
+  return trace_region_bytes(num_sms(), trace_warps(phase), events_per_warp);
+}
+
+extern "C" int b200_attn_trace_set(void* buf, size_t bytes, int events_per_warp) {
+  using namespace b200;
+  if (buf != nullptr) {
+    B200_CHECK_ARG(events_per_warp > 0, "attn_trace_set: events_per_warp must be > 0 (got %d)", events_per_warp);
+    B200_CHECK_ARG(((uintptr_t)buf % 16) == 0, "attn_trace_set: the buffer must be 16-byte aligned");
+    // The region size depends on the grid: num_sms() queries the device's SM count once (cached).  That query
+    // enqueues nothing; it is the only CUDA call made before every argument has been checked.
+    const size_t one = b200_attn_trace_launch_bytes(kTracePhaseDecode, events_per_warp);
+    B200_CHECK_ARG(bytes >= one, "attn_trace_set: buffer of %zu bytes is smaller than one launch region (%zu)", bytes,
+                   one);
+  }
+  std::lock_guard<std::mutex> lock(g_trace_mu);
+  if (buf == nullptr) {  // off; the counts stay readable until the next buffer is registered
+    g_trace.buf = nullptr;
+    g_trace_on.store(false);
+    return 0;
+  }
+  g_trace.buf = static_cast<uint8_t*>(buf);
+  g_trace.bytes = bytes;
+  g_trace.used = 0;
+  g_trace.events_per_warp = events_per_warp;
+  g_trace.traced = g_trace.untraced = 0;
+  g_trace_on.store(true);
+  return 0;
+}
+
+extern "C" int b200_attn_trace_launches(uint64_t* traced, uint64_t* untraced) {
+  using namespace b200;
+  B200_CHECK_ARG(traced != nullptr && untraced != nullptr, "attn_trace_launches: NULL output pointer");
+  std::lock_guard<std::mutex> lock(g_trace_mu);
+  *traced = g_trace.traced;
+  *untraced = g_trace.untraced;
+  return 0;
+}
+
+extern "C" int b200_abi_version(void) { return 8; }
 
 #ifndef B200_BUILD_DIGEST
 #define B200_BUILD_DIGEST "B200DIGEST:unknown"
