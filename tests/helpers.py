@@ -124,18 +124,119 @@ def poison_unowned(w: World) -> None:
     w.pool_cpu[:, :, torch.from_numpy(~used)] = float("nan")
 
 
-def make_inputs(w: World, seed: int, strided: bool = True, reqs: Optional[Sequence[Tuple[int, int, int]]] = None):
+def make_inputs(w: World, seed: int, reqs: Optional[Sequence[Tuple[int, int, int]]] = None):
     """q/k/v for the new tokens of `reqs` (default w.reqs) as row-strided views of one qkv buffer
     (layers/attention.py:49)."""
     g = torch.Generator().manual_seed(seed)
     nnz = sum(d - c for (_, c, d) in (w.reqs if reqs is None else reqs))
     width = (w.hq + 2 * w.hkv) * w.d
     qkv = torch.randn((nnz, width), generator=g, dtype=torch.float32).to(w.dtype)
-    if not strided:
-        q, k, v = [x.contiguous() for x in qkv.split([w.hq * w.d, w.hkv * w.d, w.hkv * w.d], -1)]
-    else:
-        q, k, v = qkv.split([w.hq * w.d, w.hkv * w.d, w.hkv * w.d], dim=-1)
+    q, k, v = qkv.split([w.hq * w.d, w.hkv * w.d, w.hkv * w.d], dim=-1)
     return qkv, q, k, v
+
+
+# ------------------------------------------------------------------ operand layouts
+# A layout takes the dense qkv rows [nnz, q_w + k_w + v_w] and the three widths and returns (q, k, v) as 2-D
+# row-strided views holding the same values.  Every element of the buffers behind the views that no view covers
+# is NaN (layout_padding), so a kernel that reads with the wrong row stride sees NaN or another operand's rows.
+def padded_rows(x: torch.Tensor, pad: int) -> torch.Tensor:
+    """x copied into the leading columns of a NaN buffer `pad` elements wider: row stride x.shape[1] + pad."""
+    buf = torch.full((x.shape[0], x.shape[1] + pad), float("nan"), dtype=x.dtype, device=x.device)
+    buf[:, : x.shape[1]] = x
+    return buf[:, : x.shape[1]]
+
+
+def _layout_split(qkv, widths):
+    return qkv.split(list(widths), dim=-1)
+
+
+def _layout_separate(qkv, widths):
+    return tuple(x.contiguous() for x in qkv.split(list(widths), dim=-1))
+
+
+def _layout_kv_pair(qkv, widths):
+    q, k, v = qkv.split(list(widths), dim=-1)
+    kv = torch.cat([k, v], dim=-1)
+    return q.contiguous(), kv[:, : widths[1]], kv[:, widths[1] :]
+
+
+def _layout_padded(qkv, widths, pads=(64, 128, 192)):
+    return tuple(padded_rows(x, p) for x, p in zip(qkv.split(list(widths), dim=-1), pads))
+
+
+def _layout_padded_shared_kv(qkv, widths):
+    return _layout_padded(qkv, widths, pads=(64, 128, 128))
+
+
+LAYOUTS = {
+    "split": _layout_split,  # slices of one qkv row: q_rs == k_rs == v_rs (the engine's layout)
+    "separate": _layout_separate,  # three contiguous tensors: q_rs = hq d, k_rs = v_rs = hkv d
+    "kv_pair": _layout_kv_pair,  # separate q projection, fused kv projection: k_rs == v_rs = 2 hkv d
+    "padded": _layout_padded,  # three wider buffers: q_rs, k_rs, v_rs pairwise distinct, none a dense width
+    "padded_shared_kv": _layout_padded_shared_kv,  # padded, but k and v buffers of one row stride (prefill)
+}
+
+
+def layout_padding(views: Sequence[torch.Tensor]) -> torch.Tensor:
+    """The elements of the buffers behind `views` that none of the views covers, flattened (empty for dense
+    layouts).  Every buffer must be contiguous (the layouts allocate them so)."""
+    bases, covered = {}, {}
+    for t in views:
+        b = t if t._base is None else t._base
+        assert b.is_contiguous()
+        bases[id(b)] = b
+        m = covered.setdefault(id(b), torch.zeros(b.numel(), dtype=torch.bool, device=b.device))
+        m.as_strided(t.shape, t.stride(), t.storage_offset() - b.storage_offset()).fill_(True)
+    return torch.cat([bases[i].reshape(-1)[~covered[i]] for i in bases]) if bases else torch.empty(0)
+
+
+def assert_all_nan_bits(x: torch.Tensor, what: str) -> None:
+    """Every element of x holds exactly the bits the layouts filled the padding with."""
+    nan = torch.tensor(float("nan"), dtype=x.dtype).view(torch.int16).item()
+    bits = x.cpu().view(torch.int16)
+    assert bool((bits == nan).all()), f"{what}: {(bits != nan).sum().item()} of {bits.numel()} padding elements written"
+
+
+def ulp_close(a: torch.Tensor, b: torch.Tensor, ulps: float = 1.0, scale: Optional[torch.Tensor] = None):
+    """|a-b| <= ulps * ulp(scale) elementwise for 16-bit floats (fp32 reduction-order noise only); scale
+    defaults to |b|, the result itself.  A NaN in a or b fails."""
+    a32, b32 = a.float().cpu(), b.float().cpu()
+    eps = 2.0**-8 if a.dtype == torch.bfloat16 else 2.0**-11
+    s = b32.abs() if scale is None else scale.float().cpu()
+    tol = ulps * eps * s.clamp_min(1e-3) * 2
+    bad = ~((a32 - b32).abs() <= tol)  # a NaN compares false, so it counts as bad
+    assert not bad.any(), f"{bad.sum().item()} / {bad.numel()} beyond {ulps} ulp; max {((a32-b32).abs()).max()}"
+
+
+def assert_pre_attention_close(q: Optional[torch.Tensor], k: Optional[torch.Tensor], qkv: torch.Tensor,
+                               positions: torch.Tensor, hq: int, hkv: int, d: int, cos_sin_cache: torch.Tensor,
+                               q_weight=None, k_weight=None, eps: float = 1e-6) -> None:
+    """q [nnz, hq*d] and k [nnz, hkv*d] (any device, any row stride; None = not checked) against
+    oracle.layer.ref_pre_attention of the raw rows qkv (q-norm, k-norm, neox RoPE).  Without a norm weight the
+    rows are within one ulp of the oracle.  With one, the normed value is rounded before RoPE reads it, and that
+    rounding may differ by one ulp between kernel and oracle; RoPE carries it into the output as up to one ulp of
+    each rotated term, so the bound is one ulp of |out| + |x1 cos| + |x2 sin| (x = the oracle's normed row), which
+    a cancellation cannot shrink."""
+    from oracle.layer import ref_pre_attention
+    from oracle.norm import ref_rmsnorm
+
+    qkv, positions, cos_sin_cache = qkv.cpu(), positions.cpu(), cos_sin_cache.cpu()
+    weights = [None if x is None else x.cpu() for x in (q_weight, k_weight)]
+    ref_q, ref_k, _ = ref_pre_attention(qkv, positions, hq, hkv, d, cos_sin_cache, *weights, eps)
+    nnz, half = qkv.shape[0], d // 2
+    cs = cos_sin_cache[positions.to(torch.int64)].abs().unsqueeze(1)  # [nnz, 1, d]
+    for got, ref, x, wt, heads in ((q, ref_q, qkv[:, : hq * d], weights[0], hq),
+                                   (k, ref_k, qkv[:, hq * d : (hq + hkv) * d], weights[1], hkv)):
+        if got is None:
+            continue
+        ref = ref.reshape(nnz, heads * d)
+        if wt is None:
+            ulp_close(got, ref)
+            continue
+        xn = ref_rmsnorm(x.reshape(nnz, heads, d), wt, eps).float().abs()
+        x1, x2, c, s = xn[..., :half], xn[..., half:], cs[..., :half], cs[..., half:]
+        terms = torch.cat((x1 * c + x2 * s, x2 * c + x1 * s), dim=-1).reshape(nnz, heads * d)
+        ulp_close(got, ref, scale=ref.float().abs() + terms)
 
 
 def oracle_forward(w: World, layer: int, q, k, v, md: o_meta.RefMetadata, fp32: bool = True,
@@ -293,17 +394,20 @@ class GpuWorld:
 
 
 def run_attention(gw: GpuWorld, batch, qkv: torch.Tensor, *, layer: int = 0, fused: Optional[tuple] = None,
-                  graph: bool = False, prepare: bool = True):
+                  graph: bool = False, prepare: bool = True, layout=_layout_split):
     """One attention launch of `batch` on the device rows `qkv` [nnz, (hq + 2 hkv) d], as the engine runs it:
     prepare_metadata (unless the caller ran it already: prepare=False), then `forward`, or for a decode batch
-    with fused = (cos_sin_cache, q_weight, k_weight, eps) `forward_decode_fused` on the raw q / k rows.  graph:
+    with fused = (cos_sin_cache, q_weight, k_weight, eps) `forward_decode_fused` on the raw q / k rows.  layout
+    (one of LAYOUTS) lays q, k and v out from `qkv`; the default slices one qkv row, as the engine does.  graph:
     the decode launch is captured into a CUDA graph on a dummy batch of the same size and replayed on `batch`
-    after prepare_for_replay, like the engine's graph runner.  Synchronises.  Returns (out, decode plan, pool K
+    after prepare_for_replay, like the engine's graph runner; its static q / k / v buffers come from the same
+    layout, so the captured launch sees the same strides.  Synchronises.  Returns (out, decode plan, pool K
     rows, pool V rows of the layer), all on the device."""
     w, backend = gw.w, gw.backend
+    widths = (w.hq * w.d, w.hkv * w.d, w.hkv * w.d)
 
-    def launch(x, b):
-        q, k, v = x.split([w.hq * w.d, w.hkv * w.d, w.hkv * w.d], dim=-1)
+    def launch(qkv_views, b):
+        q, k, v = qkv_views
         if fused is None:
             return backend.forward(q.view(-1, w.hq, w.d), k, v, layer, b)
         return backend.forward_decode_fused(q.view(-1, w.hq, w.d), k, v, layer, b, b.positions, *fused)
@@ -311,7 +415,7 @@ def run_attention(gw: GpuWorld, batch, qkv: torch.Tensor, *, layer: int = 0, fus
     if not graph:
         if prepare:
             backend.prepare_metadata(batch)
-        out = launch(qkv, batch)
+        out = launch(layout(qkv, widths), batch)
     else:
         # static buffers of the "graph runner", captured on a batch of dummy requests of the same size
         bs = batch.padded_size
@@ -320,22 +424,23 @@ def run_attention(gw: GpuWorld, batch, qkv: torch.Tensor, *, layer: int = 0, fus
         cap = gw.b200.Batch([dummy] * bs, "decode")
         cap.padded_reqs = cap.reqs
         backend.prepare_for_capture(cap)
-        qkv_buf = torch.zeros_like(qkv)
+        static = layout(torch.zeros_like(qkv), widths)
         cap.positions = torch.zeros(bs, dtype=torch.int32, device=gw.dev)
         cap.out_loc = torch.full((bs,), int(w.page_table[-1, 0]), dtype=torch.int32, device=gw.dev)
         out = torch.zeros(bs, w.hq, w.d, dtype=qkv.dtype, device=gw.dev)
         stream = torch.cuda.Stream()
         with torch.cuda.stream(stream):
-            out.copy_(launch(qkv_buf, cap))  # warm-up outside the capture
+            out.copy_(launch(static, cap))  # warm-up outside the capture
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, stream=stream):
-                out.copy_(launch(qkv_buf, cap))
+                out.copy_(launch(static, cap))
         torch.cuda.synchronize()
         if prepare:
             backend.prepare_metadata(batch)
         stream.wait_stream(torch.cuda.current_stream())  # the live metadata is built on the current stream
         with torch.cuda.stream(stream):
-            qkv_buf.copy_(qkv)
+            for dst, src in zip(static, qkv.split(list(widths), dim=-1)):
+                dst.copy_(src)
             cap.positions.copy_(batch.positions)
             cap.out_loc.copy_(batch.out_loc)
             backend.prepare_for_replay(batch)

@@ -6,8 +6,9 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import (GpuWorld, add_requests, assert_bits_equal, attn_tolerance_ok, check_decode_plan, make_inputs,
-                     make_world, options, oracle_forward, padded_reqs, poison_unowned, replan, run_attention)
+from helpers import (GpuWorld, add_requests, assert_bits_equal, assert_pre_attention_close, attn_tolerance_ok,
+                     check_decode_plan, make_inputs, make_world, options, oracle_forward, padded_reqs, poison_unowned,
+                     replan, run_attention)
 from oracle import metadata as o_meta
 
 pytestmark = pytest.mark.gpu
@@ -259,11 +260,17 @@ def test_prefill_unaligned_cached_boundary(b200, native_lib, page_size, prefill_
 
 
 # ------------------------------------------------------------------ fused pre-attention decode
-def _fused_vs_unfused(b200, *, page_size, hq, hkv, lens, with_norm=True, pad_to=None, seed=3, dtype=torch.bfloat16,
-                      force_split=False):
+NORMS = {"both": (True, True), "q": (True, False), "k": (False, True), "none": (False, False)}
+
+
+def _fused_vs_unfused(b200, *, page_size, hq, hkv, lens, norms="both", pad_to=None, seed=3, dtype=torch.bfloat16,
+                      force_split=False, check_oracle=False):
     """b200_attn_decode_fused (raw q / k in, qk-norm + RoPE + append + attention in ONE launch) must equal
     ops.qknorm_rope_inplace followed by backend.forward BIT FOR BIT: output, appended K/V rows, and the
-    raw q / k inputs must stay untouched."""
+    raw q / k inputs must stay untouched.  norms: which of the q / k norm weights the layer has (NORMS).
+    check_oracle: the fused output is also held to the fp32 oracle of the whole chain (q-norm, k-norm, RoPE,
+    attention), the appended k rows to one ulp of the oracle's roped rows."""
+    from oracle.layer import ref_pre_attention
     from oracle.rope import ref_cos_sin_cache
 
     max_seq = max(d for _, d in lens) + 8
@@ -274,10 +281,15 @@ def _fused_vs_unfused(b200, *, page_size, hq, hkv, lens, with_norm=True, pad_to=
     ref_md = o_meta.ref_prepare_metadata(w.page_table, reqs, page_size)
     qkv, _, _, _ = make_inputs(w, seed + 1, reqs=reqs)
     d = w.d
-    cache = ref_cos_sin_cache(d, max(4096, max_seq), 1e6).cuda()
+    cache = ref_cos_sin_cache(d, max(4096, max_seq), 1e6)
     g = torch.Generator().manual_seed(seed)
-    qw = (torch.rand(d, generator=g) + 0.5).to(dtype).cuda() if with_norm else None
-    kw = (torch.rand(d, generator=g) + 0.5).to(dtype).cuda() if with_norm else None
+    qw = (torch.rand(d, generator=g) + 0.5).to(dtype)
+    kw = (torch.rand(d, generator=g) + 0.5).to(dtype)
+    qw, kw = (x if on else None for x, on in zip((qw, kw), NORMS[norms]))
+    if check_oracle:
+        q, k, v = ref_pre_attention(qkv, torch.from_numpy(ref_md.positions), hq, hkv, d, cache, qw, kw, 1e-6)
+        ref_out, _, _ = oracle_forward(w, 0, q, k, v, ref_md, reqs=reqs)
+    cache, qw, kw = (x.cuda() if x is not None else None for x in (cache, qw, kw))
     with options(b200, **({"decode_plan_nosplit": 0} if force_split else {})):
         gw = GpuWorld(b200, w)
         batch = gw.batch("decode", pad_to=pad_to, md=ref_md)
@@ -298,6 +310,10 @@ def _fused_vs_unfused(b200, *, page_size, hq, hkv, lens, with_norm=True, pad_to=
     mask = torch.ones(k0.shape[0], dtype=torch.bool)
     mask[torch.from_numpy(ref_md.out_loc.astype(np.int64))] = False
     assert_bits_equal(k0[mask], k1[mask], "k rows nobody appended to")
+    if check_oracle:
+        attn_tolerance_ok(o1[:n_real], ref_out[:n_real], f"fused decode {dtype} vs the oracle of the chain")
+        assert_pre_attention_close(None, k1[slots].reshape(n_real, -1), qkv[:n_real],
+                                   torch.from_numpy(ref_md.positions[:n_real]), hq, hkv, d, cache, qw, kw)
 
 
 @pytest.mark.parametrize("page_size", [1, 64])
@@ -314,7 +330,7 @@ def test_decode_fused_gqa_groups(b200, native_lib, hq, hkv):
 def test_decode_fused_without_qk_norm_and_padded(b200, native_lib):
     """Llama-style layer (no q/k norm weights) and a graph-padded batch of dummy requests (kv_len 1:
     units that consist of the appended token only)."""
-    _fused_vs_unfused(b200, page_size=16, hq=8, hkv=1, lens=DECODE_LENS["mixed"][:3], with_norm=False)
+    _fused_vs_unfused(b200, page_size=16, hq=8, hkv=1, lens=DECODE_LENS["mixed"][:3], norms="none")
     _fused_vs_unfused(b200, page_size=16, hq=16, hkv=8, lens=DECODE_LENS["mixed"][:3], pad_to=8)
 
 
@@ -327,8 +343,19 @@ def test_decode_fused_split_kv_and_many_units(b200, native_lib):
     _fused_vs_unfused(b200, page_size=16, hq=16, hkv=8, lens=lens)
 
 
+@pytest.mark.parametrize("norms", ["q", "k"])
+@pytest.mark.parametrize("hq,hkv", [(8, 1), (64, 8)])
+def test_decode_fused_one_norm_weight(b200, native_lib, hq, hkv, norms):
+    """Only one of the norm weights: the Q loader norms the q rows of a group and not the k row (or the other
+    way round) in the same warp."""
+    _fused_vs_unfused(b200, page_size=16, hq=hq, hkv=hkv, lens=DECODE_LENS["mixed"][:5], norms=norms)
+
+
 def test_decode_fused_fp16(b200, native_lib):
-    _fused_vs_unfused(b200, page_size=1, hq=16, hkv=8, lens=DECODE_LENS["mixed"][:4], dtype=torch.float16)
+    """Bit-identical to the two-launch path, and both held to the fp32 oracle of the whole chain: the fp16
+    qknorm_rope_lanes is shared by the two paths, so only the oracle can tell it is right."""
+    _fused_vs_unfused(b200, page_size=1, hq=16, hkv=8, lens=DECODE_LENS["mixed"][:4], dtype=torch.float16,
+                      check_oracle=True)
 
 
 # ------------------------------------------------------------------ reference GPU goldens at real shapes

@@ -78,12 +78,12 @@ def test_decode_large_groups_graph_replay(b200, native_lib, hq, hkv, merge):
     assert_bits_equal(vc[slots], ref_vc[slots], "appended v rows")
 
 
-@pytest.mark.parametrize("with_norm", [True, False], ids=["qk-norm", "no-norm"])
+@pytest.mark.parametrize("norms", ["both", "none", "q", "k"], ids=["qk-norm", "no-norm", "q-norm", "k-norm"])
 @pytest.mark.parametrize("hq,hkv", [(9, 1), (12, 1), (16, 1), (32, 2)])
-def test_decode_fused_large_groups_bit_identical(b200, native_lib, hq, hkv, with_norm):
+def test_decode_fused_large_groups_bit_identical(b200, native_lib, hq, hkv, norms):
     """The fused launch (qk-norm + RoPE of up to 16 q rows and the k row in the Q loader) equals
-    ops.qknorm_rope_inplace followed by forward, bit for bit."""
-    _fused_vs_unfused(b200, page_size=16, hq=hq, hkv=hkv, lens=DECODE_LENS["mixed"][:5], with_norm=with_norm)
+    ops.qknorm_rope_inplace followed by forward, bit for bit, with both norm weights, none, or only one."""
+    _fused_vs_unfused(b200, page_size=16, hq=hq, hkv=hkv, lens=DECODE_LENS["mixed"][:5], norms=norms)
 
 
 @pytest.mark.parametrize("hq,hkv", [(12, 1), (16, 1)])

@@ -2,21 +2,13 @@
 import pytest
 import torch
 
+from helpers import ulp_close
 from oracle import norm as o_norm
 from oracle import rope as o_rope
 from oracle.index import ref_indexing
 from oracle.store import ref_store_kv
 
 pytestmark = pytest.mark.gpu
-
-
-def _ulp_close(a: torch.Tensor, b: torch.Tensor, ulps: float = 1.0):
-    """|a-b| <= ulps * ulp(b) elementwise for 16-bit floats (fp32 reduction-order noise only)."""
-    a32, b32 = a.float().cpu(), b.float().cpu()
-    eps = 2.0**-8 if a.dtype == torch.bfloat16 else 2.0**-11
-    tol = ulps * eps * b32.abs().clamp_min(1e-3) * 2
-    bad = (a32 - b32).abs() > tol
-    assert not bad.any(), f"{bad.sum().item()} / {bad.numel()} beyond {ulps} ulp; max {((a32-b32).abs()).max()}"
 
 
 @pytest.mark.parametrize("idx_dtype", [torch.int32, torch.int64])
@@ -134,10 +126,10 @@ def test_rmsnorm_rows(b200, native_lib, rows, dim, dtype):
     w = (torch.randn(dim) * 0.5 + 1).to(dtype)
     ref = o_norm.ref_rmsnorm(x, w, 1e-6)
     out = b200.ops.rmsnorm(x.cuda(), w.cuda(), 1e-6)
-    _ulp_close(out, ref)
+    ulp_close(out, ref)
     xg = x.cuda()
     b200.ops.rmsnorm(xg, w.cuda(), 1e-6, out=xg)  # in place (forward_inplace)
-    _ulp_close(xg, ref)
+    ulp_close(xg, ref)
 
 
 @pytest.mark.parametrize("heads,d", [(16, 128), (8, 128), (5, 64), (2, 256)])
@@ -151,7 +143,7 @@ def test_rmsnorm_per_head_strided(b200, native_lib, heads, d):
     bg = buf.cuda()
     view = bg[:, : heads * d].view(nnz, heads, d)
     b200.ops.rmsnorm(view, w.cuda(), 1e-6, out=view)
-    _ulp_close(view, ref)
+    ulp_close(view, ref)
     assert torch.equal(bg[:, heads * d :].cpu(), buf[:, heads * d :])  # neighbours untouched
 
 
@@ -185,7 +177,7 @@ def test_fused_add_rmsnorm(b200, native_lib, rows, dim, dtype, strided):
         xg, rg = x.cuda(), res.cuda()
     b200.ops.fused_add_rmsnorm(xg, rg, w.cuda(), 1e-6)
     assert torch.equal(rg.cpu().view(torch.int16), ref_res.view(torch.int16))  # residual: exact
-    _ulp_close(xg, ref_x)
+    ulp_close(xg, ref_x)
     if strided:
         assert torch.equal(xb[:, dim:], pads[0]) and torch.equal(rb[:, dim:], pads[1])
 
@@ -204,16 +196,24 @@ def test_rmsnorm_rejects_rows_wider_than_16384(b200, native_lib):
     assert b200._cabi.launch_count() == launches
     y = (torch.randn(3, 1024) * 3).to(torch.bfloat16)
     wy = (torch.randn(1024) * 0.5 + 1).to(torch.bfloat16)
-    _ulp_close(b200.ops.rmsnorm(y.cuda(), wy.cuda(), 1e-6), o_norm.ref_rmsnorm(y, wy, 1e-6))
+    ulp_close(b200.ops.rmsnorm(y.cuda(), wy.cuda(), 1e-6), o_norm.ref_rmsnorm(y, wy, 1e-6))
 
 
+def _shape_params(shapes):
+    """pytest params (*shape, dtype): bf16 under the shape's plain id, fp16 under "fp16-" + id."""
+    return [pytest.param(*shape, dtype, id=("fp16-" if dtype == torch.float16 else "") + "-".join(map(str, shape)))
+            for dtype in (torch.bfloat16, torch.float16) for shape in shapes]
+
+
+# D = 256 is the lane-group width of a whole warp (rotation partner lane j ^ 16)
 @pytest.mark.parametrize("pos_dtype", [torch.int32, torch.int64])
-@pytest.mark.parametrize("hq,hkv,d", [(16, 8, 128), (8, 1, 128), (40, 8, 128), (4, 4, 64)])
-def test_rope_neox(b200, native_lib, pos_dtype, hq, hkv, d):
+@pytest.mark.parametrize("hq,hkv,d,dtype", _shape_params([(16, 8, 128), (8, 1, 128), (40, 8, 128), (4, 4, 64),
+                                                          (4, 2, 256)]))
+def test_rope_neox(b200, native_lib, pos_dtype, hq, hkv, d, dtype):
     torch.manual_seed(11)
     nnz, max_pos = 97, 4096
     cache = o_rope.ref_cos_sin_cache(d, max_pos, 1e6)
-    qkv = torch.randn(nnz, (hq + 2 * hkv) * d).to(torch.bfloat16)
+    qkv = torch.randn(nnz, (hq + 2 * hkv) * d).to(dtype)
     pos = torch.randint(0, max_pos, (nnz,), dtype=pos_dtype)
     q, k = qkv[:, : hq * d], qkv[:, hq * d : (hq + hkv) * d]
     ref_q = o_rope.ref_apply_rope_neox(pos, q, d, cache)
@@ -222,8 +222,8 @@ def test_rope_neox(b200, native_lib, pos_dtype, hq, hkv, d):
     b200.ops.apply_rope_with_cos_sin_cache_inplace(
         positions=pos.cuda(), query=g[:, : hq * d], key=g[:, hq * d : (hq + hkv) * d],
         head_size=d, cos_sin_cache=cache.cuda())
-    _ulp_close(g[:, : hq * d], ref_q)
-    _ulp_close(g[:, hq * d : (hq + hkv) * d], ref_k)
+    ulp_close(g[:, : hq * d], ref_q)
+    ulp_close(g[:, hq * d : (hq + hkv) * d], ref_k)
     assert torch.equal(g[:, (hq + hkv) * d :].cpu(), qkv[:, (hq + hkv) * d :])  # v untouched
 
 
@@ -237,16 +237,20 @@ def test_rope_llama3_and_yarn_cache_match_oracle(b200):
     assert torch.equal(a, o_rope.ref_cos_sin_cache(128, 2048, 10000.0, sc))
 
 
-@pytest.mark.parametrize("with_norm", [True, False])
-def test_fused_qknorm_rope_equals_three_launches(b200, native_lib, with_norm):
+@pytest.mark.parametrize("with_norm,d,dtype", [
+    pytest.param(True, 128, torch.bfloat16, id="True"), pytest.param(False, 128, torch.bfloat16, id="False"),
+    *[pytest.param(with_norm, d, dtype, id=f"{with_norm}-{tag}") for tag, d, dtype in
+      (("256", 256, torch.bfloat16), ("fp16-128", 128, torch.float16), ("fp16-256", 256, torch.float16))
+      for with_norm in (True, False)]])
+def test_fused_qknorm_rope_equals_three_launches(b200, native_lib, with_norm, d, dtype):
     """The fused pre-attention launch must be bit-identical to norm -> norm -> rope."""
     torch.manual_seed(5)
-    nnz, hq, hkv, d = 130, 16, 8, 128
+    nnz, hq, hkv = 130, 16, 8
     cache = o_rope.ref_cos_sin_cache(d, 4096, 1e6).cuda()
-    qkv = torch.randn(nnz, (hq + 2 * hkv) * d).to(torch.bfloat16).cuda()
+    qkv = torch.randn(nnz, (hq + 2 * hkv) * d).to(dtype).cuda()
     pos = torch.randint(0, 4096, (nnz,), dtype=torch.int32).cuda()
-    qw = (torch.rand(d) + 0.5).to(torch.bfloat16).cuda() if with_norm else None
-    kw = (torch.rand(d) + 0.5).to(torch.bfloat16).cuda() if with_norm else None
+    qw = (torch.rand(d) + 0.5).to(dtype).cuda() if with_norm else None
+    kw = (torch.rand(d) + 0.5).to(dtype).cuda() if with_norm else None
     a, b = qkv.clone(), qkv.clone()
     qa, ka = a[:, : hq * d], a[:, hq * d : (hq + hkv) * d]
     if with_norm:
@@ -258,17 +262,18 @@ def test_fused_qknorm_rope_equals_three_launches(b200, native_lib, with_norm):
 
 
 @pytest.mark.parametrize("which", ["q_only", "k_only"])
-@pytest.mark.parametrize("d", [64, 128])
-def test_fused_qknorm_rope_mixed_weights(b200, native_lib, which, d):
+@pytest.mark.parametrize("d,dtype", _shape_params([(64,), (128,), (256,)]))
+def test_fused_qknorm_rope_mixed_weights(b200, native_lib, which, d, dtype):
     """Only one of q_weight / k_weight given: a warp then holds normed and un-normed head groups side
-    by side (2 groups per warp at D=128, 4 at D=64) -- the group reduction must not diverge."""
+    by side (2 groups per warp at D=128, 4 at D=64; at D=256 a group is the whole warp) -- the group
+    reduction must not diverge."""
     torch.manual_seed(6)
     nnz, hq, hkv = 37, 3, 1  # odd head counts: q and k groups share warps
     cache = o_rope.ref_cos_sin_cache(d, 512, 1e6).cuda()
-    qkv = torch.randn(nnz, (hq + 2 * hkv) * d).to(torch.bfloat16).cuda()
+    qkv = torch.randn(nnz, (hq + 2 * hkv) * d).to(dtype).cuda()
     pos = torch.randint(0, 512, (nnz,), dtype=torch.int32).cuda()
-    qw = (torch.rand(d) + 0.5).to(torch.bfloat16).cuda() if which == "q_only" else None
-    kw = (torch.rand(d) + 0.5).to(torch.bfloat16).cuda() if which == "k_only" else None
+    qw = (torch.rand(d) + 0.5).to(dtype).cuda() if which == "q_only" else None
+    kw = (torch.rand(d) + 0.5).to(dtype).cuda() if which == "k_only" else None
     a, b = qkv.clone(), qkv.clone()
     qa, ka = a[:, : hq * d], a[:, hq * d : (hq + hkv) * d]
     if qw is not None:
