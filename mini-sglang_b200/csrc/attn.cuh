@@ -61,7 +61,7 @@ inline DecodeWorkspace carve_decode_workspace(void* workspace, size_t workspace_
 
 // ------------------------------------------------------------------------ TMA over the KV pool
 // Rows per tiled TMA box: the largest power of two <= min(page_size, 64) that divides page_size, if that is at
-// least 8 (the slots of a page are consecutive pool rows); 0 = row mode, one single-row box per token.
+// least 8 (the slots of a page are consecutive pool rows); 0 = row mode, the pool rows are gathered with cp.async.
 inline int box_rows_for(int page_size) {
   if (page_size < 8) return 0;
   int rows = 64;
@@ -143,31 +143,51 @@ __device__ __forceinline__ UnitList<Unit, kSlotBytes, kCap, GetUnit> deal_units(
   return {slots, get, total, (total + (int)gridDim.x - 1) / (int)gridDim.x, (int)gridDim.x, (int)blockIdx.x};
 }
 
-// K/V tile geometry: a K or V tile is 128 keys x 128 dims, two 64-column halves of [128 rows x 128 B], 128B-swizzled,
-// written in place by TMA.  A producer lane fills one half of a run of keys: in box mode (page_size >= 8) a box of
-// rb consecutive keys of one page, lane = (box, half); in row mode four keys, lane = (group, half) over the 16
-// groups of a part (part 0: keys 0-63, part 1: keys 64-127).
+// K/V tile geometry: a K or V tile is 128 keys x 128 dims, two 64-column halves of [128 rows x 128 B], 128B-swizzled.
+// In box mode (page_size >= 8) TMA writes it in place, one box of rb consecutive keys of one page per producer lane,
+// lane = (box, half).  In row mode the pool keys are gathered with cp.async into the same layout (gather_part).
 constexpr int kKvTileRows = 128, kKvHalfBytes = kKvTileRows * 128, kKvTileBytes = 2 * kKvHalfBytes;
 struct KvLane {
   int row, half;  // first key of the run within the tile, 64-column half
   __device__ __forceinline__ static KvLane box(int lane, int rb) { return {(lane >> 1) * rb, lane & 1}; }
   __device__ __forceinline__ static int box_lanes(int rb) { return (kKvTileRows / rb) * 2; }  // lanes with a box
-  __device__ __forceinline__ static KvLane group(int lane, int part) { return {(part * 16 + (lane >> 1)) * 4, lane & 1}; }
   __device__ __forceinline__ uint32_t dst(uint32_t ring, uint32_t stage) const { return ring + stage * kKvTileBytes + half * kKvHalfBytes + row * 128; }
   __device__ __forceinline__ int col(int col0) const { return col0 + half * 64; }
 };
-// Slots of keys pos0 .. pos0+3 (16-byte aligned); keys at or past `end` map to num_slots, out of range (zero filled).
+// Slots of keys pos0 .. pos0+3 (16-byte aligned); keys at or past `end` map to num_slots, out of range.
 __device__ __forceinline__ int4 kv_slot_group(const int32_t* slots, int pos0, int end, int num_slots) {
   if (pos0 + 3 < end) return __ldg(reinterpret_cast<const int4*>(slots + pos0));
   auto slot = [&](int i) { return pos0 + i < end ? __ldg(slots + pos0 + i) : num_slots; };
   return make_int4(slot(0), slot(1), slot(2), slot(3));
 }
-// the four single-row boxes of a row group
-__device__ __forceinline__ void tma_load_group(uint32_t dst, const CUtensorMap* m, uint32_t bar, int col, int4 rows) {
-  sm90::tma_load_2d(dst, m, bar, col, rows.x);
-  sm90::tma_load_2d(dst + 128, m, bar, col, rows.y);
-  sm90::tma_load_2d(dst + 256, m, bar, col, rows.z);
-  sm90::tma_load_2d(dst + 384, m, bar, col, rows.w);
+// Row-mode gather (page_size < 8): keys 64 part + r, r < n, of the K or V stage at `stage` are copied from the pool
+// rows `src` + slot * row_elems (the head's 128 columns) with 16-byte cp.async, into the 128B-swizzled layout TMA
+// writes.  One warp instruction moves two 256-byte rows, keys r = i (lanes 0-15) and r = 32 + i (lanes 16-31), lane
+// & 15 being the 16-byte chunk, so eight lanes cover a 128-byte half row.  `slots` = kv_slot_group of keys 64 part +
+// 4 (lane & 15) ..: lane 8 (r / 32) + (r % 32) / 4 holds the slot of key r in component r % 4, one shuffle per
+// instruction.  A key whose slot is num_slots (past the end of the range) is zero filled and never read; keys r >= n
+// are not written.  Completion is the caller's cp_async_mbar_arrive_noinc.
+template <typename T>
+__device__ __forceinline__ void gather_part(uint32_t stage, int part, const T* src, int row_elems, int4 slots,
+                                            int num_slots, int n, int lane) {
+  // Rolled over 8-key atoms (a full unroll costs the producers registers they do not have): key r = r_hi + 8 a + k
+  // sits at byte (part 64 + r) 128 of its half, chunk j ^ k (sw128_offset with row & 7 = k).
+  const int j = lane & 15, r_hi = (lane >> 4) * 32, lane0 = (lane >> 4) * 8;
+  const uint32_t dst0 = stage + (j >> 3) * kKvHalfBytes + (part * 64 + r_hi) * 128;
+  const T* src_j = src + j * 8;
+#pragma unroll 1
+  for (int a = 0; a < 4; ++a) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int c = (k & 3) == 0 ? slots.x : (k & 3) == 1 ? slots.y : (k & 3) == 2 ? slots.z : slots.w;
+      const int s = __shfl_sync(0xffffffffu, c, lane0 + 2 * a + (k >> 2));
+      if (r_hi + 8 * a + k < n) {
+        const bool in = s < num_slots;
+        sm90::cp_async_16(dst0 + a * 1024 + k * 128 + (((j ^ k) & 7) << 4), src_j + (in ? (int64_t)s * row_elems : 0),
+                          in ? 16u : 0u);
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------ event trace

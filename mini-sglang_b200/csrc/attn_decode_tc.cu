@@ -4,16 +4,19 @@
 // with one persistent launch (+ the split-KV combine).  HBM-bound; algorithmic bytes as in
 // attn_decode_bringup.cu.  One CTA per SM, 320 threads, warp-specialised:
 //
-//   warps 0-3 TMA producers, 3-stage rings of 32 KB K and 32 KB V tiles (two 64-column halves of a
+//   warps 0-3 producers, 3-stage rings of 32 KB K and 32 KB V tiles (two 64-column halves of a
 //            128-key tile), data lands directly in the 128-byte-swizzled layout wgmma consumes.
 //            * page_size >= 8 ("box mode", warp 0 = K, warp 1 = V): the slots of a page are contiguous
 //              rows of the pool, so one tiled TMA box of min(page_size, 64) rows x 128 B is issued per
 //              page piece -- 4 instructions per tile and half at page_size 64.  The piece holding the
 //              end of the KV range is loaded as 8-row boxes up to its last valid row, and pieces past
 //              the end are not loaded at all, so no more than 7 rows past the end come from HBM.
-//            * page_size < 8 ("row mode", all four warps): one single-row TMA box per token row and
-//              half; rows past the end of the KV range are out-of-range rows (zero filled), so stale
-//              pool memory is never multiplied in.
+//            * page_size < 8 ("row mode", warps 0,1 = K keys 0-63 / 64-127, warps 2,3 = V): a warp-wide
+//              cp.async gather, 16 bytes per lane, two 256-byte token rows per instruction (gather_part);
+//              rows past the end of the KV range are zero filled and never read, so stale pool memory is
+//              never multiplied in.  Every producer lane arrives on the stage's full barrier once its copies
+//              have landed (cp.async.mbarrier.arrive.noinc: 64 arrivals, no transaction bytes), and every
+//              consumer thread fences the generic-proxy writes for the tensor core after its wait.
 //   warps 4-7 one consumer warpgroup: S^T[128 keys x N] = K_tile . Q^T and O^T[128 dims x N] += V_tile^T . P^T
 //            as wgmma m64nNk16 (two 64-row blocks each): the keys / head dims fill M and the query heads of
 //            the GQA group sit in N -- N = 8 for groups of 1-8, N = 16 for groups of 9-16, chosen at compile
@@ -111,7 +114,7 @@ struct Params {
   float* part_ml;
   int* counters;  // [bs][hkv] split-KV arrival counters, zero between launches
   // fused pre-attention (fuse = 1): q / k_new are raw; norm weights may be NULL (models without qk-norm)
-  int early;  // 1: captured launch -- TMA producers do not wait for the predecessor (see the kernel prologue)
+  int early;  // 1: captured launch -- K/V producers do not wait for the predecessor (see the kernel prologue)
   int fuse;
   const T* qw;
   const T* kw;
@@ -157,11 +160,10 @@ __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_
 }
 
 // kTrace: each warp records its events into p.trace (attn.cuh); the false instantiation is the product kernel.
-template <typename T, int G, bool kTrace>
+// kRows: row mode (p.box_rows == 0), a separate instantiation so that box mode's tile loop carries none of it.
+template <typename T, int G, bool kTrace, bool kRows>
 __global__ void __launch_bounds__(kThreads, 1)
-attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map_k,
-                      const __grid_constant__ CUtensorMap map_v,
-                      const __grid_constant__ CUtensorMap box_k,
+attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap box_k,
                       const __grid_constant__ CUtensorMap box_v,
                       const __grid_constant__ CUtensorMap tail_k,
                       const __grid_constant__ CUtensorMap tail_v) {
@@ -183,10 +185,12 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   for (int i = tid; i < (2 * Smem::kQBufBytes) / 16; i += kThreads)
     reinterpret_cast<uint4*>(smem + Smem::qbuf)[i] = make_uint4(0, 0, 0, 0);
   if (tid == 0) {
+    // full: box mode, lane 0's expect_tx; row mode, every lane of the two warps that gather the tile
+    const uint32_t n_fill = kRows ? 2 * kWarp : 1;
     for (int s = 0; s < kStages; ++s) {
-      mbar_init(bar(kFullK + s), 1);
+      mbar_init(bar(kFullK + s), n_fill);
       mbar_init(bar(kEmptyK + s), 4);  // one elected arrival per consumer warp
-      mbar_init(bar(kFullV + s), 1);
+      mbar_init(bar(kFullV + s), n_fill);
       mbar_init(bar(kEmptyV + s), 4);
     }
     for (int b = 0; b < kFinRing; ++b) {
@@ -202,12 +206,12 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
       mbar_init(bar(kQEmpty + b), 4);
     }
     fence_barrier_init();
-    prefetch_tensormap(&map_k);
-    prefetch_tensormap(&map_v);
-    prefetch_tensormap(&box_k);
-    prefetch_tensormap(&box_v);
-    prefetch_tensormap(&tail_k);
-    prefetch_tensormap(&tail_v);
+    if constexpr (!kRows) {  // row mode passes no tensor maps
+      prefetch_tensormap(&box_k);
+      prefetch_tensormap(&box_v);
+      prefetch_tensormap(&tail_k);
+      prefetch_tensormap(&tail_v);
+    }
   }
   // PDL: everything above may overlap the tail of the previous kernel in the stream.
   //  * p.early == 0 (eager launches): wait here -- from here on the results of every kernel before this one
@@ -216,7 +220,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   //    (prepare_for_replay), and the K/V rows this launch streams belong to this layer's pool slice, which
   //    no other kernel of the graph writes -- so only the roles that consume the predecessor's outputs
   //    (Q loader: q / k_new; consumer warps: v_new, out_loc operands, output / partial stores; combiner)
-  //    wait, while the TMA producers start streaming K/V at once: prologue, pipeline fill and the
+  //    wait, while the K/V producers start streaming K/V at once: prologue, pipeline fill and the
   //    predecessor's tail (or a small kernel in between, e.g. the TP all-reduce) overlap.
   if (!p.early) pdl_wait();
   pdl_launch_dependents();
@@ -233,7 +237,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   fence_proxy_async_smem();  // zero-fill above must be visible to wgmma operand reads
   __syncthreads();
   if (warp < 4) {
-    // ============================================================ TMA producers
+    // ============================================================ K/V producers
     // K and V travel in separate rings (a K tile is dead as soon as QK^T has completed, a V
     // tile only after PV), so each has its own producers: box mode warp 0 = K, warp 1 = V;
     // row mode warps 0,1 = K rows 0-63 / 64-127, warps 2,3 = V.
@@ -242,7 +246,6 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
     if (rb > 0 && warp >= 2) {
       // box mode needs a handful of instructions per tile: two warps are plenty
     } else {
-      const CUtensorMap* gmap = kind == 0 ? &map_k : &map_v;
       const CUtensorMap* bmap = kind == 0 ? &box_k : &box_v;
       const int full0 = kind == 0 ? kFullK : kFullV, empty0 = kind == 0 ? kEmptyK : kEmptyV;
       const uint32_t ring = sbase + (kind == 0 ? Smem::kring : Smem::vring);
@@ -258,22 +261,23 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
         }
         const int32_t* slots = p.slot_table + (int64_t)u.r * p.st_stride;
         const int col0 = u.h * kD;
-        if (rb == 0) {
-          // ---- row mode: this warp owns 64 rows
-          const KvLane L = KvLane::group(lane, warp & 1);
-          auto load_group = [&](int t) {
-            return kv_slot_group(slots, u.kv_begin + t * kKvTileRows + L.row, u.kv_end_tc, p.num_slots);
+        if constexpr (kRows) {
+          // ---- row mode: this warp gathers keys 64 part .. 64 part + 63 of every tile
+          const int part = warp & 1;
+          const T* src = (kind == 0 ? p.k_cache : p.v_cache) + col0;
+          auto load_slots = [&](int t) {
+            return kv_slot_group(slots, u.kv_begin + t * kKvTileRows + part * 64 + 4 * (lane & 15), u.kv_end_tc,
+                                 p.num_slots);
           };
-          int4 nxt = load_group(0);
+          int4 nxt = load_slots(0);
           for (int t = 0; t < u.n_tiles; ++t, kv.advance()) {
             const int4 cur = nxt;
-            if (t + 1 < u.n_tiles) nxt = load_group(t + 1);
+            if (t + 1 < u.n_tiles) nxt = load_slots(t + 1);
             tr.ev(kEvEmptyWait, t);
             kv.wait_empty(bar(empty0));
             tr.ev(kEvEmptyDone, t);
-            if ((warp & 1) == 0 && lane == 0) mbar_arrive_expect_tx(bar(full0 + kv.stage()), kKvTileBytes);
-            __syncwarp();
-            tma_load_group(L.dst(ring, kv.stage()), gmap, bar(full0 + kv.stage()), L.col(col0), cur);
+            gather_part(ring + kv.stage() * kKvTileBytes, part, src, p.hkv * kD, cur, p.num_slots, 64, lane);
+            cp_async_mbar_arrive_noinc(bar(full0 + kv.stage()));
             tr.ev(kEvIssued, t);
           }
         } else {
@@ -460,6 +464,13 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           const uint32_t stage = kv.stage();
           // ---- S^T = K_tile . Q^T: A = K rows (K-major, 128B swizzle), B = Q rows (K-major, 8-row atoms 1024 B apart)
           kv.wait_full(bar(kFullK));
+          // Row mode: the tile was written by cp.async, generic-proxy writes, and wgmma reads it through the async
+          // proxy.  The full barrier's phase completes only after every copy of the tile has landed (each producer
+          // lane's arrival waits for its own copies), so the writes happen before this thread's wait returns; the
+          // fence then orders them before this thread's async-proxy reads.  The producers cannot fence: they never
+          // wait for their copies.  (Overwriting a slot after the release below needs no fence: wgmma_wait0 has
+          // completed the reads before the release, and the next copies are issued after it.)
+          if constexpr (kRows) fence_proxy_async_smem();
           tr.ev(kEvKFull, j);
           const uint32_t kb = sbase + Smem::kring + stage * kKvTileBytes;
           float s[2][N / 2];
@@ -552,6 +563,7 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
           tr.ev(kEvSoftmax, j);
           // ---- O^T += V_tile^T . P^T: A = V rows read MN-major, B = P^T (K-major, no swizzle)
           kv.wait_full(bar(kFullV));
+          if constexpr (kRows) fence_proxy_async_smem();  // as for the K tile
           tr.ev(kEvVFull, j);
           const uint32_t vb = sbase + Smem::vring + stage * kKvTileBytes;
           const uint32_t pb = sbase + Smem::pbuf;
@@ -798,31 +810,34 @@ attn_decode_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map
   tr.finish();
 }
 
-template <typename T, int G, bool kTrace>
-static int launch_kernel(const Params<T>& p, const CUtensorMap& mk, const CUtensorMap& mv, const CUtensorMap& bk,
-                         const CUtensorMap& bv, const CUtensorMap& tk, const CUtensorMap& tv, cudaStream_t st) {
+template <typename T, int G, bool kTrace, bool kRows>
+static int launch_kernel(const Params<T>& p, const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& tk,
+                         const CUtensorMap& tv, cudaStream_t st) {
   const size_t smem = Smem<kNOf<G>>::total + 1024;
   static bool configured = false;
   if (!configured) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_decode_tc_kernel<T, G, kTrace>,
+    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_decode_tc_kernel<T, G, kTrace, kRows>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(attn_decode_tc_kernel<T, G, kTrace>, dim3(num_sms()), dim3(kThreads), smem, st, p, mk, mv,
-                             bk, bv, tk, tv));
+  B200_CHECK_CUDA(launch_pdl(attn_decode_tc_kernel<T, G, kTrace, kRows>, dim3(num_sms()), dim3(kThreads), smem, st, p, bk, bv,
+                             tk, tv));
   return 0;
 }
 
 template <typename T, int G>
-static int launch_g(Params<T> p, const CUtensorMap& mk, const CUtensorMap& mv,
-                    const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& tk,
+static int launch_g(Params<T> p, const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& tk,
                     const CUtensorMap& tv, cudaStream_t st) {
   // a registered trace buffer with a region left selects the instrumented instantiation (same launch otherwise)
   if (trace_next_region(kTracePhaseDecode, num_sms(), &p.trace)) {
     p.trace.flags = (p.fuse ? kTraceFused : 0u) | (p.fused_combine ? kTraceInKernelCombine : 0u) | (p.early ? kTraceEarlyKv : 0u);
-    if (int rc = launch_kernel<T, G, true>(p, mk, mv, bk, bv, tk, tv, st)) return rc;
+    if (int rc = p.box_rows == 0 ? launch_kernel<T, G, true, true>(p, bk, bv, tk, tv, st)
+                                 : launch_kernel<T, G, true, false>(p, bk, bv, tk, tv, st))
+      return rc;
   } else {
-    if (int rc = launch_kernel<T, G, false>(p, mk, mv, bk, bv, tk, tv, st)) return rc;
+    if (int rc = p.box_rows == 0 ? launch_kernel<T, G, false, true>(p, bk, bv, tk, tv, st)
+                                 : launch_kernel<T, G, false, false>(p, bk, bv, tk, tv, st))
+      return rc;
   }
   B200_POST_LAUNCH();
   if (!p.fused_combine) {
@@ -853,9 +868,7 @@ static int launch(const DecodeArgs& a) {
                     (const T*)a.qw, (const T*)a.kw, a.eps, a.positions, a.cos_sin,
                     TraceArgs{nullptr, 0, 0, a.page_size, 0}};
   const bool bf16 = std::is_same<T, __nv_bfloat16>::value;
-  CUtensorMap mk, mv;
-  if (int rc = kv_pool_maps(&mk, &mv, a.k_cache, a.v_cache, a.num_slots, a.hkv, 1, bf16)) return rc;
-  CUtensorMap bk = mk, bv = mv;
+  CUtensorMap bk{}, bv{};  // row mode gathers with cp.async and needs no tensor map
   if (p.box_rows > 0)
     if (int rc = kv_pool_maps(&bk, &bv, a.k_cache, a.v_cache, a.num_slots, a.hkv, p.box_rows, bf16)) return rc;
   // 8-row boxes for the last page piece of a range (exact tail)
@@ -863,22 +876,22 @@ static int launch(const DecodeArgs& a) {
   if (p.box_rows > 8)
     if (int rc = kv_pool_maps(&tk, &tv, a.k_cache, a.v_cache, a.num_slots, a.hkv, 8, bf16)) return rc;
   switch (p.hq / p.hkv) {
-    case 1: return launch_g<T, 1>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 2: return launch_g<T, 2>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 3: return launch_g<T, 3>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 4: return launch_g<T, 4>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 5: return launch_g<T, 5>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 6: return launch_g<T, 6>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 7: return launch_g<T, 7>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 8: return launch_g<T, 8>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 9: return launch_g<T, 9>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 10: return launch_g<T, 10>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 11: return launch_g<T, 11>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 12: return launch_g<T, 12>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 13: return launch_g<T, 13>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 14: return launch_g<T, 14>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 15: return launch_g<T, 15>(p, mk, mv, bk, bv, tk, tv, a.stream);
-    case 16: return launch_g<T, 16>(p, mk, mv, bk, bv, tk, tv, a.stream);
+    case 1: return launch_g<T, 1>(p, bk, bv, tk, tv, a.stream);
+    case 2: return launch_g<T, 2>(p, bk, bv, tk, tv, a.stream);
+    case 3: return launch_g<T, 3>(p, bk, bv, tk, tv, a.stream);
+    case 4: return launch_g<T, 4>(p, bk, bv, tk, tv, a.stream);
+    case 5: return launch_g<T, 5>(p, bk, bv, tk, tv, a.stream);
+    case 6: return launch_g<T, 6>(p, bk, bv, tk, tv, a.stream);
+    case 7: return launch_g<T, 7>(p, bk, bv, tk, tv, a.stream);
+    case 8: return launch_g<T, 8>(p, bk, bv, tk, tv, a.stream);
+    case 9: return launch_g<T, 9>(p, bk, bv, tk, tv, a.stream);
+    case 10: return launch_g<T, 10>(p, bk, bv, tk, tv, a.stream);
+    case 11: return launch_g<T, 11>(p, bk, bv, tk, tv, a.stream);
+    case 12: return launch_g<T, 12>(p, bk, bv, tk, tv, a.stream);
+    case 13: return launch_g<T, 13>(p, bk, bv, tk, tv, a.stream);
+    case 14: return launch_g<T, 14>(p, bk, bv, tk, tv, a.stream);
+    case 15: return launch_g<T, 15>(p, bk, bv, tk, tv, a.stream);
+    case 16: return launch_g<T, 16>(p, bk, bv, tk, tv, a.stream);
     default:  // attn_decode() has refused every other group size
       set_error("attn_decode: GQA group size %d not supported by the wgmma decode kernel (1..%d)", p.hq / p.hkv,
                 kMaxGroup);

@@ -7,8 +7,10 @@
 // tile, query head); the query heads of one kv head are adjacent units, so neighbouring CTAs stream the
 // same K/V rows and the re-reads hit in L2.
 //
-//   warp 0      K producer (+ the unit's Q tile): TMA boxes per page piece / single-row boxes
-//   warp 1      V producer
+//   warp 0      K producer (+ the unit's Q tile), warp 1 V producer.  This forward's own keys come from the
+//               k / v inputs in TMA boxes; pool keys in TMA boxes per page piece (page_size >= 8) or, at
+//               page_size < 8, in a warp-wide cp.async gather (gather_part), which the consumers fence for
+//               the tensor core after their wait, as in the decode kernel
 //   (append)    fused KV append: the producers write the tile of a unit that holds the unit's own new
 //               tokens to the pool straight from shared memory (TMA store); the attention reads this
 //               forward's tokens from the k / v inputs, never back from the pool, so no ordering is needed
@@ -98,7 +100,9 @@ __device__ __forceinline__ uint32_t pack2(float lo, float hi) {
 }
 
 // kTrace: each warp records its events into p.trace (attn.cuh); the false instantiation is the product kernel.
-template <typename T, bool kTrace>
+// kRows: row mode (p.box_rows == 0).  The two load modes are separate instantiations so that the producers' 40
+// registers hold only the state of one of them.
+template <typename T, bool kTrace, bool kRows>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap map_q,
                        const __grid_constant__ CUtensorMap map_k,
@@ -107,7 +111,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
                        const __grid_constant__ CUtensorMap box_v,
                        const __grid_constant__ CUtensorMap new_k,    // k input rows, box {64, 1}
                        const __grid_constant__ CUtensorMap new_v,
-                       const __grid_constant__ CUtensorMap newbox_k, // k input rows, box {64, box_rows}
+                       const __grid_constant__ CUtensorMap newbox_k, // k input rows, box {64, box_rows or 64}
                        const __grid_constant__ CUtensorMap newbox_v) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -127,10 +131,12 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
   // ---------------------------------------------------------------- one-time setup
   units.stage(tid, kThreads);
   if (tid == 0) {
+    // full: lane 0's expect_tx, and in row mode every lane of the producer warp once its gather has landed
+    const uint32_t n_fill = kRows ? 1 + kWarp : 1;
     for (int s = 0; s < kStages; ++s) {
-      mbar_init(bar(kFullK + s), 1);
+      mbar_init(bar(kFullK + s), n_fill);
       mbar_init(bar(kEmptyK + s), 8);  // one elected arrival per consumer warp
-      mbar_init(bar(kFullV + s), 1);
+      mbar_init(bar(kFullV + s), n_fill);
       mbar_init(bar(kEmptyV + s), 8);
     }
     mbar_init(bar(kQFull), 1);
@@ -154,7 +160,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
   if (warp < 4) {
    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
    if (warp < 2) {
-    // ============================================================ TMA producers: warp 0 = K (+Q), warp 1 = V
+    // ============================================================ producers: warp 0 = K (+Q), warp 1 = V
     const int kind = warp;
     const int rb = p.box_rows;
     const CUtensorMap* gmap = kind == 0 ? &map_k : &map_v;
@@ -179,7 +185,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
     auto issue_stores = [&](int stage) {  // whole warp; the tile has landed
       Pending& pd = pend[stage];
       tr.ev(kEvAppend, pd.tile_begin / kKvTileRows);
-      if (rb > 0) {
+      if constexpr (!kRows) {
         if (lane < KvLane::box_lanes(rb)) {
           const KvLane L = KvLane::box(lane, rb);
           const int pb = pd.tile_begin + L.row;
@@ -193,14 +199,11 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
           }
         }
       } else {
-#pragma unroll
-        for (int it = 0; it < 2; ++it) {
-          const KvLane L = KvLane::group(lane, it);
-          const int pos0 = pd.tile_begin + L.row;
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            if (pos0 + i >= pd.lo && pos0 + i < pd.hi)
-              tma_store_2d(smap_row, L.dst(ring, stage) + i * 128, L.col(pd.col0), __ldg(pd.slots + pos0 + i));
+        // one single-row store per appended key and half
+        for (int i = lane; i < 2 * (pd.hi - pd.lo); i += kWarp) {
+          const int pos = pd.lo + (i >> 1), half = i & 1;
+          tma_store_2d(smap_row, ring + stage * kKvTileBytes + half * kKvHalfBytes + (pos - pd.tile_begin) * 128,
+                       pd.col0 + half * 64, __ldg(pd.slots + pos));
         }
       }
       bulk_commit();
@@ -261,7 +264,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
         const uint32_t stage = kv.stage();
         const uint32_t fb = bar(full0 + stage);
         const int tile_begin = t * kKvTileRows;
-        if (rb > 0) {
+        if constexpr (!kRows) {
           const int n_instr = KvLane::box_lanes(rb);
           const KvLane L = KvLane::box(lane, rb);
           const int pb = tile_begin + L.row;
@@ -282,22 +285,33 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
             else load_rows_one_by_one(dst, fb, col, pb, rb);  // the box straddling cached_len
           }
         } else {
-          // row mode: 32 row groups of four x 2 halves = 2 groups per lane, one single-row box per row
+          // row mode: keys [tile_begin, tile_begin + n_pool) are pool keys, gathered with cp.async; the keys of this
+          // forward follow, in 64-row input boxes and one row at a time in the box that straddles cached_len
+          const int n_pool = min(max(u.cached - tile_begin, 0), kKvTileRows);
+          const int new0 = (n_pool + 63) & ~63;  // first key of the input boxes
           tr.ev(kEvEmptyWait, t);
           kv.wait_empty(bar(empty0));
           tr.ev(kEvEmptyDone, t);
           flush_stage(stage);
-          if (lane == 0) mbar_arrive_expect_tx(fb, kKvTileBytes);
+          if (lane == 0) mbar_arrive_expect_tx(fb, (uint32_t)(kKvTileRows - n_pool) * 256u);
           __syncwarp();
-#pragma unroll
-          for (int it = 0; it < 2; ++it) {
-            const KvLane L = KvLane::group(lane, it);
-            const int pos0 = tile_begin + L.row;
-            if (pos0 + 4 <= u.cached)
-              tma_load_group(L.dst(ring, stage), gmap, fb, L.col(col0), kv_slot_group(slots, pos0, u.cached, p.num_slots));
-            else
-              load_rows_one_by_one(L.dst(ring, stage), fb, L.col(col0), pos0, 4);
+          const uint32_t dst = ring + stage * kKvTileBytes;
+          if (lane < 4 && (lane >> 1) * 64 >= new0)
+            tma_load_2d(dst + (lane & 1) * kKvHalfBytes + (lane >> 1) * 64 * 128, nbmap, fb, col0 + (lane & 1) * 64,
+                        u.q_begin + tile_begin + (lane >> 1) * 64 - u.cached);
+          for (int i = lane; i < 2 * (new0 - n_pool); i += kWarp) {
+            const int row = n_pool + (i >> 1), half = i & 1;
+            tma_load_2d(dst + half * kKvHalfBytes + row * 128, nmap, fb, col0 + half * 64,
+                        u.q_begin + tile_begin + row - u.cached);
           }
+          const T* src = (kind == 0 ? p.k_cache : p.v_cache) + col0;
+#pragma unroll 1
+          for (int part = 0; part < 2; ++part)
+            if (n_pool > part * 64)
+              gather_part(dst, part, src, p.hkv * kD,
+                          kv_slot_group(slots, tile_begin + part * 64 + 4 * (lane & 15), u.cached, p.num_slots),
+                          p.num_slots, n_pool - part * 64, lane);
+          cp_async_mbar_arrive_noinc(fb);
         }
         tr.ev(kEvIssued, t);
         if (kind == 0 && t == 0) load_q();
@@ -360,6 +374,9 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
         const int tile_begin = j * kKvTileRows;
         const bool active = tile_begin < wg_vis;  // warpgroup-uniform
         kv.wait_full(bar(kFullK));
+        // row mode: the gathered pool keys are generic-proxy writes that have landed before the wait returned;
+        // order them before this thread's wgmma reads (attn_decode_tc.cu gives the argument)
+        if constexpr (kRows) fence_proxy_async_smem();
         tr.ev(kEvKFull, j);
         float s[64];
         if (active) {
@@ -428,6 +445,7 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
           tr.ev(kEvSoftmax, j);
         }
         kv.wait_full(bar(kFullV));
+        if constexpr (kRows) fence_proxy_async_smem();
         tr.ev(kEvVFull, j);
         if (active) {
           const uint32_t vb = sbase + Smem::vring + stage * kKvTileBytes;
@@ -474,18 +492,18 @@ attn_prefill_tc_kernel(const Params<T> p, const __grid_constant__ CUtensorMap ma
   tr.finish();
 }
 
-template <typename T, bool kTrace>
+template <typename T, bool kTrace, bool kRows>
 static int launch_kernel(const Params<T>& p, cudaStream_t st, const CUtensorMap& mq, const CUtensorMap& mk,
                          const CUtensorMap& mv, const CUtensorMap& bk, const CUtensorMap& bv, const CUtensorMap& nk,
                          const CUtensorMap& nv, const CUtensorMap& nbk, const CUtensorMap& nbv) {
   const size_t smem = Smem::total + 1024;
   static bool configured = false;
   if (!configured) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_tc_kernel<T, kTrace>,
+    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_prefill_tc_kernel<T, kTrace, kRows>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = true;
   }
-  attn_prefill_tc_kernel<T, kTrace><<<num_sms(), kThreads, smem, st>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
+  attn_prefill_tc_kernel<T, kTrace, kRows><<<num_sms(), kThreads, smem, st>>>(p, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
   B200_POST_LAUNCH();
   return 0;
 }
@@ -508,15 +526,18 @@ static int launch(const PrefillArgs& a) {
   // move between forwards)
   if (int rc = encode_tensor_map_2d(&nk, p.k_new, a.nnz, cols, p.kv_rs * 2, 64, 1, bf16)) return rc;
   if (int rc = encode_tensor_map_2d(&nv, p.v_new, a.nnz, cols, p.kv_rs * 2, 64, 1, bf16)) return rc;
-  CUtensorMap nbk = nk, nbv = nv;
-  if (p.box_rows > 0) {
-    if (int rc = encode_tensor_map_2d(&nbk, p.k_new, a.nnz, cols, p.kv_rs * 2, 64, p.box_rows, bf16)) return rc;
-    if (int rc = encode_tensor_map_2d(&nbv, p.v_new, a.nnz, cols, p.kv_rs * 2, 64, p.box_rows, bf16)) return rc;
-  }
+  // ... and in boxes: of the pool's box rows, or of 64 rows in row mode
+  const uint32_t new_rows = p.box_rows > 0 ? p.box_rows : 64;
+  CUtensorMap nbk, nbv;
+  if (int rc = encode_tensor_map_2d(&nbk, p.k_new, a.nnz, cols, p.kv_rs * 2, 64, new_rows, bf16)) return rc;
+  if (int rc = encode_tensor_map_2d(&nbv, p.v_new, a.nnz, cols, p.kv_rs * 2, 64, new_rows, bf16)) return rc;
   // a registered trace buffer with a region left selects the instrumented instantiation (same launch otherwise)
-  if (trace_next_region(kTracePhasePrefill, num_sms(), &p.trace))
-    return launch_kernel<T, true>(p, a.stream, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
-  return launch_kernel<T, false>(p, a.stream, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
+  const bool traced = trace_next_region(kTracePhasePrefill, num_sms(), &p.trace);
+  if (p.box_rows == 0)
+    return traced ? launch_kernel<T, true, true>(p, a.stream, mq, mk, mv, bk, bv, nk, nv, nbk, nbv)
+                  : launch_kernel<T, false, true>(p, a.stream, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
+  return traced ? launch_kernel<T, true, false>(p, a.stream, mq, mk, mv, bk, bv, nk, nv, nbk, nbv)
+                : launch_kernel<T, false, false>(p, a.stream, mq, mk, mv, bk, bv, nk, nv, nbk, nbv);
 }
 
 }  // namespace ptc

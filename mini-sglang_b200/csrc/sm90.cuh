@@ -103,6 +103,18 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
+// ------------------------------------------------------------------------------ cp.async (16-byte gathers)
+// 16 bytes global -> shared through L2 only; src_bytes = 0 reads nothing and zero fills the 16 bytes.  The write is
+// a generic-proxy write: wgmma / TMA may read it only after a fence.proxy.async that follows its completion.
+__device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(src), "r"(src_bytes) : "memory");
+}
+// One arrival on `bar` once every cp.async this thread has issued so far has completed.  .noinc: the arrival is one
+// of those the barrier was initialised to expect (its pending count is not raised first).
+__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
+
 // ------------------------------------------------------------------------------ wgmma
 // A warpgroup (4 consecutive warps, the first a multiple of 4) issues every wgmma together.  The
 // accumulator fragment of m64nN: warp w of the group, lane l holds rows 16w + l/4 (+8) and columns
