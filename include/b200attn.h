@@ -149,6 +149,18 @@ B200_API int b200_qknorm_rope_inplace(void* q, void* k, const void* q_weight, co
                              void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * K8  Gated-MLP activation.  Replaces flashinfer.silu_and_mul(x, out=...) at M/layers/activation.py:9-13,
+ *     called by GatedMLP.forward (M/models/utils.py:33,48) in every decoder layer of the dense models.
+ *     x viewed as [rows, 2d], out as [rows, d]; row strides in elements (x_row_stride >= 2d,
+ *     out_row_stride >= d), last dim contiguous, any d in [1, 2^30].
+ *     out[t, i] = round(silu(x[t, i]) * x[t, d + i]) with FlashInfer's fast-math arithmetic (ex2.approx,
+ *     div.approx, flush-to-zero fp32), bit for bit.  16-byte vectors when d % 8 == 0 and every row is
+ *     16-byte aligned, one element per thread otherwise.  rows == 0 launches nothing.
+ * ------------------------------------------------------------------------------------- */
+B200_API int b200_silu_and_mul(void* out, int64_t out_row_stride, const void* x, int64_t x_row_stride,
+                               int64_t rows, int d, int dtype, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * a2/a3/a4  Metadata on device.  Replaces the host loops of prepare_metadata
  *     (M/attention/fa.py:67-105, fi.py:190-225): from per-request triples
  *     req_info[bs][3] = (table_idx, cached_len, device_len) (int32; device memory or PINNED host memory,

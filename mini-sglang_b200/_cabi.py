@@ -14,7 +14,7 @@ from typing import Optional
 _LIB: Optional[C.CDLL] = None
 LIB_PATH = Path(__file__).resolve().parent / "libb200attn.so"
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 _i32, _i64, _f32, _vp, _sz = C.c_int, C.c_int64, C.c_float, C.c_void_p, C.c_size_t
 
@@ -41,6 +41,7 @@ SIGNATURES = {
         _i32,
         [_vp, _vp, _vp, _vp, _f32, _vp, _i32, _vp, _i64, _i32, _i32, _i32, _i64, _i64, _i32, _vp],
     ),
+    "b200_silu_and_mul": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _i32, _vp]),
     "b200_decode_plan_ints": (_sz, [_i32]),
     "b200_build_prefill_plan": (_i32, [_vp, _i32, _vp, _i32, _vp]),
     "b200_build_metadata": (

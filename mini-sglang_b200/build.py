@@ -21,6 +21,7 @@ LIB_PATH = PKG_DIR / "libb200attn.so"
 SOURCES = [
     "capi.cu",
     "elementwise.cu",
+    "activation.cu",
     "index_rows.cu",
     "metadata.cu",
     "attn_decode_bringup.cu",

@@ -129,7 +129,7 @@ extern "C" int b200_attn_trace_launches(uint64_t* traced, uint64_t* untraced) {
   return 0;
 }
 
-extern "C" int b200_abi_version(void) { return 8; }
+extern "C" int b200_abi_version(void) { return 9; }
 
 #ifndef B200_BUILD_DIGEST
 #define B200_BUILD_DIGEST "B200DIGEST:unknown"

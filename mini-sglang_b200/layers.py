@@ -296,19 +296,22 @@ _FLASHINFER_SAVED: Dict[str, Callable] = {}
 
 
 def patch_flashinfer_entry_points() -> int:
-    """Point ``flashinfer.rmsnorm`` / ``fused_add_rmsnorm`` / ``apply_rope_with_cos_sin_cache_inplace``
-    at the sm_90a ops.  The reference's layers import these names from the ``flashinfer`` package
-    inside ``__init__`` (layers/norm.py:10,25, layers/rotary.py:35), so calling this BEFORE the model is
-    built (``LLM(...)`` / ``Engine(...)``) makes every norm / rotary layer bind our kernels -- including
-    inside the decode CUDA graphs, which are captured during ``Engine.__init__`` (engine/engine.py:100,
-    engine/graph.py:105-141; re-binding layer attributes afterwards only affects eager forwards).
-    Returns the number of re-bound names; :func:`restore_flashinfer_entry_points` undoes it."""
+    """Point the FlashInfer elementwise entry points ``flashinfer.rmsnorm`` / ``fused_add_rmsnorm`` /
+    ``apply_rope_with_cos_sin_cache_inplace`` / ``silu_and_mul`` at the sm_90a ops.  The reference's layers
+    import the norm / rotary names from the ``flashinfer`` package inside ``__init__`` (layers/norm.py:10,25,
+    layers/rotary.py:35) and ``silu_and_mul`` at every call (layers/activation.py:9-13, the gated MLP of every
+    dense model), so calling this BEFORE the model is built (``LLM(...)`` / ``Engine(...)``) makes every norm /
+    rotary layer and every MLP activation run our kernels -- including inside the decode CUDA graphs, which are
+    captured during ``Engine.__init__`` (engine/engine.py:100, engine/graph.py:105-141; re-binding layer
+    attributes afterwards only affects eager forwards).  Returns the number of re-bound names;
+    :func:`restore_flashinfer_entry_points` undoes it."""
     import flashinfer
 
     table = {
         "rmsnorm": ops.rmsnorm,
         "fused_add_rmsnorm": ops.fused_add_rmsnorm,
         "apply_rope_with_cos_sin_cache_inplace": ops.apply_rope_with_cos_sin_cache_inplace,
+        "silu_and_mul": ops.silu_and_mul,
     }
     for name, fn in table.items():
         _FLASHINFER_SAVED.setdefault(name, getattr(flashinfer, name))
@@ -318,15 +321,16 @@ def patch_flashinfer_entry_points() -> int:
 
 def install_into_minisgl(norm_rope: bool = True, row_gather: bool = True, attention: bool = True) -> bool:
     """One call, before ``LLM(...)`` / ``Engine(...)``: makes the reference build its model with the sm_90a
-    norm / RoPE kernels, fuse the pre-attention work of its attention layers into the b200 launches and use
-    the sm_90a row gather, with zero edits to the reference.
+    norm / RoPE / MLP-activation kernels, fuse the pre-attention work of its attention layers into the b200
+    launches and use the sm_90a row gather, with zero edits to the reference.
 
     ``Engine.__init__`` asserts that CUDA is not initialised yet (engine/engine.py:31) and importing
     ``flashinfer`` initialises it, so the FlashInfer names cannot be re-bound up front.  Instead the module
     attribute ``minisgl.engine.engine.create_model`` (engine.py:12, called at engine.py:50-51 after the device
     is set and before the decode graphs are captured at engine.py:100) is wrapped: the wrapper re-binds the
-    FlashInfer entry points (:func:`patch_flashinfer_entry_points`, ``norm_rope``), calls the reference's own
-    ``create_model`` and re-binds ``forward`` of the model's attention layers (:func:`patch_minisgl_attention`,
+    FlashInfer elementwise entry points (:func:`patch_flashinfer_entry_points`, ``norm_rope``: RMSNorm, RoPE
+    and the gated MLP's SiLU-and-mul; with ``norm_rope=False`` all of them stay FlashInfer's), calls the
+    reference's own ``create_model`` and re-binds ``forward`` of the model's attention layers (:func:`patch_minisgl_attention`,
     ``attention``).  So with ``attention_backend="b200"`` every decode step inside the engine's CUDA graphs is
     ONE launch per layer (q-norm + k-norm + RoPE + KV append + attention); layers whose batch another backend
     serves keep their own forward.  Returns False when the reference is not importable."""

@@ -11,6 +11,7 @@ reference call site                                     function here
 ``flashinfer.apply_rope_with_cos_sin_cache_inplace``     :func:`apply_rope_with_cos_sin_cache_inplace`
 (layers/rotary.py:35,45-51)
 (the three pre-attention launches, attention.py:50-54)   :func:`qknorm_rope_inplace`
+``flashinfer.silu_and_mul`` (layers/activation.py:9-13)   :func:`silu_and_mul`
 =====================================================  =====================================
 
 Tensors are borrowed (``data_ptr``), work is enqueued on ``torch.cuda.current_stream()`` and
@@ -184,6 +185,43 @@ def fused_add_rmsnorm(
         ),
         "b200_fused_add_rmsnorm",
     )
+
+
+def silu_and_mul(
+    input: torch.Tensor, out: Optional[torch.Tensor] = None, enable_pdl: Optional[bool] = None
+) -> torch.Tensor:
+    """``flashinfer.silu_and_mul`` semantics and signature (reference layers/activation.py:9-13):
+    ``silu(input[..., :d]) * input[..., d:]`` for ``input`` of shape ``(..., 2d)``, bit for bit what FlashInfer
+    computes.  Any ``d >= 1`` and any leading dims whose rows are evenly strided; the last dim must be
+    contiguous.  ``out`` (shape ``(..., d)``, same dtype) may be row-strided.  ``enable_pdl`` is accepted for
+    signature compatibility: like every kernel of this library, the launch uses programmatic dependent launch
+    unless the library option ``use_pdl`` is 0."""
+    _require_cuda(input, out)
+    if input.dim() < 1 or input.shape[-1] % 2:
+        raise RuntimeError(f"silu_and_mul: last dim must be even, got shape {tuple(input.shape)}")
+    d = input.shape[-1] // 2
+    if out is None:
+        out = torch.empty(input.shape[:-1] + (d,), device=input.device, dtype=input.dtype)
+    elif out.shape != input.shape[:-1] + (d,) or out.dtype != input.dtype or out.device != input.device:
+        raise RuntimeError(f"silu_and_mul: out must be {tuple(input.shape[:-1]) + (d,)} of {input.dtype}")
+    if out.numel() == 0:
+        return out
+    if input.stride(-1) != 1 or out.stride(-1) != 1:
+        raise RuntimeError("silu_and_mul: the last dim of input and out must be contiguous")
+    try:
+        x2, o2 = input.view(-1, 2 * d), out.view(-1, d)
+    except RuntimeError:
+        raise RuntimeError("silu_and_mul: the leading dims of input / out must collapse to one row stride") from None
+    rows = x2.shape[0]
+    xrs = x2.stride(0) if rows > 1 else 2 * d  # the stride of a single row is never used
+    ors = o2.stride(0) if rows > 1 else d
+    _cabi.check(
+        _cabi.load().b200_silu_and_mul(
+            o2.data_ptr(), ors, x2.data_ptr(), xrs, rows, d, _dtype_code(input), _stream_ptr(input)
+        ),
+        "b200_silu_and_mul",
+    )
+    return out
 
 
 def _qk_views(query: torch.Tensor, key: torch.Tensor, head_size: int):

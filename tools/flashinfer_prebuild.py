@@ -7,6 +7,8 @@ Modules = exactly what the reference's call sites instantiate for Qwen3-0.6B / b
   fi.py:93-103  BatchPrefill/BatchDecode wrappers, backend "fa2", NHD, pos_encoding NONE
   trtllm.py:52-53 trtllm_batch_{context,decode}_with_kv_cache  (TRT-LLM-gen launcher; kernels are cubins)
   rotary.py:35  apply_rope_with_cos_sin_cache_inplace ; norm.py:10,25 rmsnorm / fused_add_rmsnorm
+  activation.py:10 silu_and_mul (GatedMLP.forward, models/utils.py:48)
+The target is the H100 (9.0a) unless FLASHINFER_CUDA_ARCH_LIST says otherwise.
 """
 import os
 import sys
@@ -15,10 +17,11 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 WS = ROOT / "oracle" / "_ref" / "flashinfer_ws"
 os.environ["FLASHINFER_WORKSPACE_BASE"] = str(WS)
-os.environ.setdefault("FLASHINFER_CUDA_ARCH_LIST", "10.0a")
+os.environ.setdefault("FLASHINFER_CUDA_ARCH_LIST", "9.0a")
 os.environ.setdefault("MAX_JOBS", str(os.cpu_count() or 8))
 
 import torch  # noqa: E402
+from flashinfer.jit.activation import gen_act_and_mul_module  # noqa: E402
 from flashinfer.jit.attention.modules import gen_batch_decode_module, gen_batch_prefill_module  # noqa: E402
 from flashinfer.jit.norm import gen_norm_module  # noqa: E402
 from flashinfer.jit.rope import gen_rope_module  # noqa: E402
@@ -29,6 +32,7 @@ specs = [
     gen_batch_prefill_module("fa2", bf, bf, bf, torch.int32, 128, 128, 0, False, False, False),
     gen_rope_module(),
     gen_norm_module(),
+    gen_act_and_mul_module("silu"),
 ]
 try:
     from flashinfer.jit.attention.modules import gen_trtllm_gen_fmha_module

@@ -10,6 +10,8 @@ forward (prefill, chunked prefill, radix-hit extend, graph-replayed padded decod
   driver mode (spawns the children, compares, prints + writes a JSON summary):
       python tools/insitu.py run --out insitu_summary.json
   `run_fused()` spawns the children of tests/test_gpu_insitu_fused.py (`--patch fused` against `--patch model`).
+  census mode (which kernels one eager prefill forward and one decode graph replay launch, torch.profiler):
+      python tools/insitu.py census --out census.json
 
 What the reference is asked to do (reference file:line of the code that runs):
   * `LLM.generate` twice (llm/llm.py:81-98): round A fills the radix cache, round B re-uses two of
@@ -64,6 +66,38 @@ def workload():
     return [a, b]
 
 
+# ------------------------------------------------------------------------------------ census
+KERNEL_GROUPS = ("ours", "cublas", "flashinfer", "other")
+
+
+def kernel_group(name: str) -> str:
+    """ours (namespace b200 of libb200attn) / cuBLAS / FlashInfer / other (PyTorch's own kernels, copies)."""
+    low = name.lower()
+    if "b200::" in name:
+        return "ours"
+    if "flashinfer" in low:
+        return "flashinfer"
+    if any(k in low for k in ("cublas", "gemm", "nvjet", "xmma", "cutlass")):
+        return "cublas"
+    return "other"
+
+
+def profile_kernels(fn):
+    """Run fn() under torch.profiler with CUDA activities; returns (fn's result, {group: {kernel: launches}})."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        result = fn()
+        torch.cuda.synchronize()
+    groups = {g: {} for g in KERNEL_GROUPS}
+    for e in prof.events():
+        if str(e.device_type).endswith("CUDA"):
+            kinds = groups[kernel_group(e.name)]
+            kinds[e.name] = kinds.get(e.name, 0) + 1
+    return result, groups
+
+
 # ------------------------------------------------------------------------------------- child
 class _StubTokenizer:
     eos_token_id = -1
@@ -104,6 +138,10 @@ def child(args) -> None:
 
     real_runner = ref_engine.GraphRunner
     forwards = {"prefill": 0, "decode": 0}  # model forwards that launch kernels: eager or being captured
+    census = {}
+
+    def launch_count():
+        return int(minisgl_b200.PACKAGE._cabi.launch_count()) if "minisgl_b200" in sys.modules else 0
 
     def runner_with_patched_model(*a, **kw):
         model = kw["model"]
@@ -118,7 +156,13 @@ def child(args) -> None:
         real_model_forward = model.forward
 
         def counted_forward(*fa, **fkw):  # graph replays do not call it
-            forwards[ref_ctx().batch.phase] += 1
+            phase = ref_ctx().batch.phase
+            forwards[phase] += 1
+            if args.census and phase == "prefill" and "prefill_forward" not in census:
+                before = launch_count()
+                out, census["prefill_forward"] = profile_kernels(lambda: real_model_forward(*fa, **fkw))
+                census["prefill_forward_b200_launches"] = launch_count() - before
+                return out
             return real_model_forward(*fa, **fkw)
 
         model.forward = counted_forward
@@ -147,6 +191,21 @@ def child(args) -> None:
         be = eng.attn_backend
         assert isinstance(be, BaseAttnBackend), "b200 backend is not a reference BaseAttnBackend"
         assert type(be).__module__.startswith("mini-sglang_b200"), type(be)
+
+    if args.census:
+        real_replay, real_sample = eng.graph_runner.replay, eng.sampler.sample
+
+        def replay(batch):
+            if "decode_replay" in census:
+                return real_replay(batch)
+            logits, census["decode_replay"] = profile_kernels(lambda: real_replay(batch))
+            census["decode_replay_bs"] = [int(batch.size), int(batch.padded_size)]
+            # the engine's own sampler on these logits, outside the forward (its result is not used)
+            sargs = eng.sampler.prepare(batch)
+            _, census["sampler"] = profile_kernels(lambda: real_sample(logits, sargs))
+            return logits
+
+        eng.graph_runner.replay = replay
 
     forced = torch.load(args.force)["tokens"] if args.force else None
     state = {"round": 0, "count": {}}
@@ -208,6 +267,8 @@ def child(args) -> None:
     torch.save({"records": records, "tokens": tokens_out, "append_keys": keys, "kv": kv,
                 "b200_launches": launches, "forwards": forwards, "args": vars(args)}, args.out)
     print(f"[insitu] {len(records)} forwards recorded, b200 kernel launches: {launches}", flush=True)
+    if args.census:
+        Path(args.census).write_text(json.dumps(census, indent=1))
     try:
         llm.shutdown()
     except Exception as e:  # pragma: no cover
@@ -276,7 +337,7 @@ def logits_bit_identical(path_a: str, path_b: str) -> bool:
 
 def run_child(tag: str, out_dir: Path, attn: str, page_size: int, force: "str | None", patch: str = "none",
               patch_kernels: bool = False, layers: int = 28, timeout: int = 600, fi_tensor_cores: bool = False,
-              unfused_attention: bool = False) -> str:
+              unfused_attention: bool = False, census: "str | None" = None) -> str:
     out = out_dir / f"{tag}.pt"
     cmd = [sys.executable, str(Path(__file__).resolve()), "child", "--attn", attn, "--page-size", str(page_size),
            "--out", str(out), "--patch", patch, "--layers", str(layers)]
@@ -288,6 +349,8 @@ def run_child(tag: str, out_dir: Path, attn: str, page_size: int, force: "str | 
         cmd += ["--fi-tensor-cores"]
     if unfused_attention:
         cmd += ["--unfused-attention"]
+    if census:
+        cmd += ["--census", census]
     t0 = time.time()
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, timeout=timeout, cwd=str(ROOT))
     log = res.stdout.decode(errors="replace")
@@ -373,6 +436,41 @@ def run_fused(args) -> dict:
     return runs
 
 
+def run_census(args) -> dict:
+    """Kernel census of the installed engine (`install_into_minisgl()`, b200 attention, page 64): every kernel of
+    one eager prefill forward and of one decode graph replay, grouped ours / cuBLAS / FlashInfer / other, and the
+    engine's sampler on that step's logits, reported apart (it runs after the forward).  The same engine with the
+    model patched layer by layer (`--patch fused`, which leaves `flashinfer.silu_and_mul` bound) is the
+    comparison: the installed prefill forward makes exactly one b200 launch more per layer (the MLP activation)."""
+    out_dir = Path(tempfile.mkdtemp(prefix="insitu_census_"))
+    L = args.layers
+    summary = {"model": f"Qwen3-0.6B shape, {L} layers, dummy weights, bf16, attention_backend=b200, page 64"}
+    for tag, patch in (("installed", "flashinfer"), ("patched_layers", "fused")):
+        path = out_dir / f"{tag}.json"
+        run_child(tag, out_dir, "b200", 64, None, patch=patch, patch_kernels=True, layers=L, census=str(path))
+        summary[tag] = json.loads(path.read_text())
+    inst, ref = summary["installed"], summary["patched_layers"]
+
+    def count(groups, group):
+        return sum(groups[group].values())
+
+    summary["checks"] = {
+        "installed_forward_flashinfer_kernels": count(inst["prefill_forward"], "flashinfer")
+        + count(inst["decode_replay"], "flashinfer"),
+        "installed_prefill_b200_launches_minus_patched_layers": inst["prefill_forward_b200_launches"]
+        - ref["prefill_forward_b200_launches"],
+        "layers": L,
+    }
+    c = summary["checks"]
+    c["ok"] = c["installed_forward_flashinfer_kernels"] == 0 and c[
+        "installed_prefill_b200_launches_minus_patched_layers"] == L
+    if args.out:
+        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+        Path(args.out).write_text(json.dumps(summary, indent=1))
+    print(json.dumps(summary, indent=1))
+    return summary
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     sub = ap.add_subparsers(dest="mode", required=True)
@@ -389,13 +487,17 @@ def main() -> None:
                    help="--patch flashinfer: install_into_minisgl(attention=False)")
     c.add_argument("--patch-kernels", action="store_true")
     c.add_argument("--fi-tensor-cores", action="store_true")
+    c.add_argument("--census", default=None, help="write the kernel census of this engine to this JSON file")
     r = sub.add_parser("run")
     r.add_argument("--out", default=None)
     r.add_argument("--layers", type=int, default=28)
+    k = sub.add_parser("census")
+    k.add_argument("--out", default=None)
+    k.add_argument("--layers", type=int, default=28)
     args = ap.parse_args()
     if not reference_available():
         raise SystemExit("the reference is not installed: MINISGL_REFERENCE=<reference checkout> python -m oracle.reference_site")
-    child(args) if args.mode == "child" else run(args)
+    {"child": child, "run": run, "census": run_census}[args.mode](args)
 
 
 if __name__ == "__main__":
